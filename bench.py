@@ -2,7 +2,7 @@
 """bench.py -- rays/sec of the layered ray-march hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--precision exact|exact_cf|mixed|fp32|fast]
-                    [--workload taekwondo2|walking4|walking6_4k] [--no-extra] [--no-cpu-baseline]
+                    [--workload taekwondo2|walking4|walking6_4k] [--no-extra] [--no-cpu-baseline] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): taekwondo 2-layer scene, 1080p, 16 views, 64 coarse + 128 fine samples.
 A *step* renders one 1080p view (2 073 600 rays; view = step mod 16) through the whole hot path: ray generation ->
@@ -16,6 +16,9 @@ value  = device-resident throughput: cameras/rays already on the device, CUDA ev
          N ranks: each view's rows are interleaved over the ranks, every rank's compositing kernel writes its pixels straight
          into its slot of a persistent all-gather buffer and ONE in-place all-gather per view assembles the fine images on
          every rank (strong scaling: total work per step is fixed).
+--dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step computed as DIR/<name>.npy (float32): the
+         fine and coarse images (rgb, depth, acc per layer + the merged image) at a fixed seeded sample of up to 262 144 pixels, and
+         the sampled pixel indices (float64).  The inputs depend only on the arguments, so two builds can be compared output by output.
 e2e    = same metric through the host-buffer C-ABI call (stnerf_render_host): pinned host rays -> H2D (chunk-pipelined) ->
          render -> D2H of every image plane (chunk-pipelined), inside the timed region, same K steps.
 --impl reference : the UNMODIFIED reference (`LayeredRFRender.forward`, run out of process from the archive packed by
@@ -56,10 +59,11 @@ WORKLOADS = {
                         name="walking 6-layer 4K, 32 views, 64+192 samples (BASELINE configs[4])"),
 }
 PRECISION_TERMS = {"exact": 3.0, "exact_cf": 3.0, "mixed": 3.0 - 2.0 * (256 * 128) / 462336.0, "fast": 1.0, "fp32": 1.0}
-DTYPES = {"exact": "f32 via fp16x3 split products (tcgen05), f32 accumulate", "fp32": "f32",
-          "exact_cf": "f32 via fp16x3 split products (tcgen05), correction products first in the coarse pass and the MotionNets, f32 accumulate", "fast": "f16 products, f32 accumulate",
+DTYPES = {"exact": "f32 via fp16x3 split products (wgmma), f32 accumulate", "fp32": "f32",
+          "exact_cf": "f32 via fp16x3 split products (wgmma), correction products first in the coarse pass and the MotionNets, f32 accumulate", "fast": "f16 products, f32 accumulate",
           "mixed": "f32 via fp16x3 split products on everything the density depends on, single f16 pass on the colour-only layer "
-                   "rgb_net.1 (tcgen05), f32 accumulate"}
+                   "rgb_net.1 (wgmma), f32 accumulate"}
+DUMP_PIXELS = 262144          # seeded pixel sample of --dump-outputs, fewer when 2 passes x planes x 5 floats would pass 60 MB
 
 
 def load_weights(wl):
@@ -82,7 +86,7 @@ def scene_setup(wl):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -231,7 +235,22 @@ def cpu_leg_parity(wl, model, dev, precision="exact"):
                        "instability of the reference) in tests/test_gpu_parity_scale.py" % wl["fixture"]}
 
 
-def measure(wl, precision, steps, warmup, rank, world, local_rank, want_e2e=True, parity_fn=None):
+def dump_outputs(dump_dir, svr, rows, H, W, world):
+    """What the last timed step returned (fine images of every layer + merged, and the coarse ones) at a seeded pixel sample."""
+    import numpy as np
+    import torch
+    os.makedirs(dump_dir, exist_ok=True)
+    n = min(DUMP_PIXELS, H * W, (60 << 20) // (2 * rows.shape[1] * 5 * 4))
+    idx = torch.randperm(H * W, generator=torch.Generator().manual_seed(20240607))[:n].sort().values
+    fine = svr.assembled(rows)[0].reshape(rows.shape[1], H * W, 5)             # (l+1, H*W, 5): rgb, depth, acc
+    np.save(os.path.join(dump_dir, "pixel_index.npy"), idx.numpy().astype(np.float64))
+    np.save(os.path.join(dump_dir, "fine_images.npy"), fine[:, idx.to(fine.device)].float().cpu().numpy())
+    if world == 1:                     # the coarse images stay on the rank that rendered them: complete on a single GPU only
+        coarse = svr._coarse[1][0].reshape(rows.shape[1], -1, 5)[:, :H * W]
+        np.save(os.path.join(dump_dir, "coarse_images.npy"), coarse[:, idx.to(coarse.device)].float().cpu().numpy())
+
+
+def measure(wl, precision, steps, warmup, rank, world, local_rank, want_e2e=True, parity_fn=None, dump_dir=None):
     """One workload on this process' GPU (all ranks call it).  Returns a dict of measurements (complete on rank 0)."""
     import torch
     import torch.distributed as dist
@@ -272,9 +291,10 @@ def measure(wl, precision, steps, warmup, rank, world, local_rank, want_e2e=True
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     coll_ms = []
+    rows = None
     e0.record()
     for i in range(steps):
-        step(warmup + i)
+        rows = step(warmup + i)
         if world > 1:
             coll_ms.append(svr._timing)
     e1.record()
@@ -285,6 +305,8 @@ def measure(wl, precision, steps, warmup, rank, world, local_rank, want_e2e=True
     prof = nat.profile_end()
     launches = S.launch_count() - launches0
     clk = clocks.stop()
+    if dump_dir is not None and rank == 0 and rows is not None:
+        dump_outputs(dump_dir, svr, rows, H, W, world)
     t = torch.tensor([ms_total], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -337,7 +359,7 @@ def measure(wl, precision, steps, warmup, rank, world, local_rank, want_e2e=True
 def roofline_of(wl, res, precision, steps, peaks):
     prof, n_local = res["prof"], res["n_local"]
     N1, N2, LAYERS = wl["n1"], wl["n2"], wl["layers"]
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
     sp = prof["spacenet"]
     # algorithmic FLOPs: 2*MAC per evaluated point (nets with a PE(time) input have the wider rgb head); the split between
     # background and performer points comes from the per-launch point counts
@@ -347,23 +369,16 @@ def roofline_of(wl, res, precision, steps, peaks):
     flops = bk_pts * FLOP_SPACE_NOTIME + max(0.0, pts - bk_pts) * flop_perf
     ach = flops / (sp["ms"] * 1e-3) / 1e12 if sp["ms"] > 0 else 0.0
     terms = PRECISION_TERMS[precision]
-    traffic, traffic_note = None, None
-    try:      # DRAM bytes per point of the same kernel from the committed `ncu --set full` capture, scaled to the mean launch
-        cap = json.load(open(os.path.join(ROOT, "profiles", "r02_spacenet_traffic.json")))
-        traffic = cap["dram_bytes_per_point"] * pts / max(1, sp["launches"])
-        traffic_note = ("NOT measured in this run: dram__bytes_read+write per point (%.1f B) from the committed ncu --set full capture "
-                        "profiles/r02_spacenet_traffic.json (%s) x this run's mean points per launch" % (cap["dram_bytes_per_point"], cap["kernel"]))
-    except Exception:
-        pass
     ms_total = res["ms_per_step"] * steps
     roof = {"kernel": "spacenet MLP (%s)" % precision, "bound": "tensor", "achieved": ach, "peak": peak_tf,
             "unit": "TFLOP/s", "frac": ach / peak_tf, "executed": ach * terms, "frac_executed": ach * terms / peak_tf,
-            "peak_source": ("measured bf16_tflops_sustained (MEASURED_PEAKS.json)" if peaks else "fallback 1400 (B200_PROFILING.md)"),
-            "traffic": traffic, "traffic_note": traffic_note, "launches": sp["launches"], "avg_launch_ms": sp["ms"] / max(1, sp["launches"]),
+            "peak_source": ("measured bf16_tflops_sustained (MEASURED_PEAKS.json)" if peaks else
+                            "H100 SXM data sheet, dense BF16/FP16 at 700 W (not a sustained rate)"),
+            "launches": sp["launches"], "avg_launch_ms": sp["ms"] / max(1, sp["launches"]),
             "share_of_step": sp["ms"] / ms_total,
             "note": "achieved/frac = algorithmic FLOPs (2*MAC/point x points evaluated) / CUDA-event launch durations of this run; the split modes "
                     "execute %.2f fp16 MMAs per product (frac = frac_executed / %.2f); executed/frac_executed = what the tensor pipe runs -- the "
-                    "denominator is a cuBLAS rate SUSTAINED UNDER THE POWER CAP, not the silicon peak, so frac_executed may pass 1" % (terms, terms),
+                    "denominator is the peak in peak_source" % (terms, terms),
             "other_kernels_ms": {k: v["ms"] for k, v in prof.items() if k != "spacenet"}}
     # compositing + resampling kernels: algorithmic bytes (depths + raw rgb-sigma in, depths + images out) against the HBM peak,
     # reported for completeness -- they are instruction-issue-bound (sort / search / scan per sample), see DESIGN.md
@@ -371,7 +386,7 @@ def roofline_of(wl, res, precision, steps, peaks):
     hit_frac = max(0.0, pts - bk_pts) / max(1.0, bk_pts)
     bytes_comp = float(n_local) * steps * ((1 + hit_frac) * (N1 * 24 + (N1 + N2) * 20 + (N1 + N2) * 4) + (LAYERS + 2) * 40)
     roof["composite_hbm"] = {"achieved_GBps": bytes_comp / (cp["ms"] * 1e-3) / 1e9 if cp["ms"] > 0 else 0.0,
-                             "peak_GBps": peaks.get("hbm_gbs", 6650.0), "share_of_step": cp["ms"] / ms_total}
+                             "peak_GBps": peaks.get("hbm_gbs", 3350.0), "share_of_step": cp["ms"] / ms_total}
     return roof
 
 
@@ -386,6 +401,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the short runs of the other BASELINE configs")
     ap.add_argument("--workload", default="taekwondo2", choices=list(WORKLOADS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's images (seeded pixel sample) as DIR/<name>.npy")
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -396,7 +413,7 @@ def main():
               "layers": wl["layers"] + 1, "n1": wl["n1"], "n2": wl["n2"],
               "parallelism": "rows interleaved over %d GPU(s); compositing kernel writes into the rank's slot of a persistent buffer; "
                              "1 in-place all-gather of the fine images per view" % world,
-              "l2": "no explicit flush: per-chunk working set (~1.2 GB of samples/raw rgb-sigma buffers) >> 126 MB L2"}
+              "l2": "no explicit flush: per-chunk working set (~1.2 GB of samples/raw rgb-sigma buffers) >> 50 MB L2"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -419,7 +436,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
     # the reference-fixture parity check belongs to the CPU leg: rank 0 of a single-GPU run, unless --no-cpu-baseline
     parity_fn = cpu_leg_parity if (world == 1 and not args.no_cpu_baseline) else None
-    res = measure(wl, args.precision, args.steps, args.warmup, rank, world, local_rank, parity_fn=parity_fn)
+    res = measure(wl, args.precision, args.steps, args.warmup, rank, world, local_rank, parity_fn=parity_fn, dump_dir=args.dump_outputs)
 
     extra = {}
     if not args.no_extra and args.workload == "taekwondo2":

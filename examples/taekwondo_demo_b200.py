@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The edit sessions of the reference's demo/taekwondo_demo.py (origin / shift / scale) on the B200 path.
+"""The edit sessions of the reference's demo/taekwondo_demo.py (origin / shift / scale) on the native H100 path.
 
 The dataset (images, point clouds, camera files) is not shipped with the reference, so the scene geometry and the 16
 ground-truth cameras are the synthetic rig of SURVEY 8(d); everything else follows the demo line by line:
@@ -16,7 +16,7 @@ import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "st-nerf_b200"))      # ahead of a reference checkout: B200 modeling/utils/layers/engine
+sys.path.insert(0, os.path.join(ROOT, "st-nerf_b200"))      # ahead of a reference checkout: native modeling/utils/layers/engine
 
 import torch                                                  # noqa: E402
 

@@ -1,5 +1,5 @@
 /*
- * stnerf.h -- C ABI of libstnerf_b200.so: the st-nerf layered ray-march hot path on B200 (sm_100a).
+ * stnerf.h -- C ABI of libstnerf_b200.so: the st-nerf layered ray-march hot path on H100 (sm_90a).
  *
  * The reference (DarlingHang/st-nerf) has no FFI seam: its boundary is the Python call surface
  *   modeling/layered_rfrender.py:141   LayeredRFRender.forward(rays, labels, bboxes, only_coarse, ...)
@@ -43,18 +43,17 @@ enum {
 /* Arithmetic mode of the two MLPs (modeling/spacenet.py:101-160, modeling/motion_net.py:34-71). */
 enum {
   STNERF_PREC_FP32_SIMT = 0,   /* fp32 FFMA on CUDA cores: the bit-closest mode, validation baseline      */
-  STNERF_PREC_TC_3XF16 = 1,    /* tcgen05 fp16 3-term split (hi*hi + lo*hi + hi*lo), fp32 accumulate:     */
+  STNERF_PREC_TC_3XF16 = 1,    /* wgmma fp16 3-term split (hi*hi + lo*hi + hi*lo), fp32 accumulate:       */
                                /* ~fp32 products, meets the 1e-3 RGB gate (SURVEY App. C.3)               */
-  STNERF_PREC_TC_F16 = 2,      /* tcgen05 single fp16 pass: fastest, does NOT meet the 1e-3 gate          */
+  STNERF_PREC_TC_F16 = 2,      /* wgmma single fp16 pass: fastest, does NOT meet the 1e-3 gate            */
   STNERF_PREC_TC_MIXED = 3,    /* TC_3XF16 for everything the density depends on (SpaceNet trunk + sigma head, MotionNet); */
                                /* single fp16 pass for the colour-only layer rgb_net.1 (spacenet.py:81-86): ~5 % fewer     */
                                /* MMAs, colour error <= 2.5e-4, resampling untouched -- inside the 1e-3 gate               */
   STNERF_PREC_TC_3XF16_CF = 4  /* TC_3XF16 with the two correction products of every layer issued FIRST (over the whole K  */
                                /* range, then hi*hi) in the coarse pass and the MotionNets -- what the sample placement    */
-                               /* depends on.  The tensor core truncates when it adds into its fp32 accumulator; this      */
-                               /* order truncates at full magnitude K/16 instead of 3K/16 times: sigma error / 3 (2e-6 rel */
-                               /* rms, the reference's own fp32 noise is 1e-6), about half the rays over the 1e-3 gate at  */
-                               /* scale; the hi weight stages stream twice (cost: see DESIGN 3.1)                          */
+                               /* depends on.  The correction terms are added while the accumulator is still small, so     */
+                               /* the tensor core's rounding of its fp32 accumulation acts on them less; the hi weight     */
+                               /* stages stream twice (see DESIGN 3.1)                                                     */
 };
 
 typedef struct stnerf_ctx* stnerf_handle;
@@ -213,21 +212,14 @@ int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, i
 int stnerf_weights_export(stnerf_handle h, void* host_buf, size_t capacity, size_t* bytes_needed);
 int stnerf_weights_import(stnerf_handle h, const void* host_buf, size_t bytes);
 
-/* Tensor-core plumbing self-test: one 128x128x64 fp16 UMMA through the library's descriptors, swizzled layout, bulk
- * copy and TMEM load; writes max |D - host reference| (expected < 1e-3).                                     */
+/* Tensor-core plumbing self-test: one 128x256x64 fp16 product through the library's warpgroup-MMA descriptors, swizzled
+ * layouts, bulk copy and accumulator fragment; writes max |D - host reference| (expected < 1e-3).                           */
 int stnerf_selftest_umma(float* max_err_host);
-/* Accumulation probe: the same 128x256x64 product of all-POSITIVE fp16 operands accumulated `reps` times into one TMEM
+/* Accumulation probe: the same 128x256x64 product of all-POSITIVE fp16 operands accumulated `reps` times into one register
  * accumulator (4*reps MMAs of K=16).  Reports max |D - fp64 sum| and the mean SIGNED relative error: how the tensor core
  * rounds when it adds into an fp32 accumulator (a negative mean growing with reps = round-toward-zero accumulation), which
  * bounds how close the fp16x3 split can get to the reference's fp32 GEMMs (DESIGN.md 4).                          */
 int stnerf_selftest_umma_accum(int reps, float* max_err_host, float* mean_signed_rel_err_host);
-/* The same through the CTA-pair protocol (`tcgen05.mma.cta_group::2`, M = 256 over the two CTAs of a cluster: remote mbarrier
- * arrives, multicast commit, paired TMEM allocation): one 256x256x64 product; expected < 1e-3.                 */
-/* The same 128x256x64 product with the A operand in TENSOR memory: written with tcgen05.st in the layout the SpaceNet epilogue
- * uses for the next layer's activations (8 columns of fp16 pairs per K=16 step at a 16-column pitch), read by
- * tcgen05.mma [d], [a], b-desc.  Pins that layout on the device the library runs on. */
-int stnerf_selftest_umma_ts(float* max_err_host);
-int stnerf_selftest_umma_pair(float* max_err_host);
 
 /* Diagnostic read-back of the sample depths of the LAST chunk rendered by stnerf_render (parity tooling: which depths did
  * utils/sample_pdf.py:18-63 + the sort of modeling/layered_rfrender.py:462 produce for these rays?).

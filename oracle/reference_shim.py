@@ -50,7 +50,7 @@ def modules():
         # the two must never be mixed in one interpreter.
         for name in ("modeling", "layers", "utils", "engine"):
             if name in sys.modules and REFERENCE_ROOT not in (getattr(sys.modules[name], "__file__", "") or ""):
-                raise RuntimeError("module %r already imported from the B200 facade; "
+                raise RuntimeError("module %r already imported from the native facade; "
                                    "run reference-driving code in a separate process" % name)
         sys.path.insert(0, REFERENCE_ROOT)
         import io

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Run the UNMODIFIED reference `LayeredRFRender.forward` (modeling/layered_rfrender.py:141) on CPU, in its own process.
 
-TEST INFRASTRUCTURE ONLY.  The B200 facade packages reuse the reference's top-level import names (`modeling`, `utils`,
+TEST INFRASTRUCTURE ONLY.  The native facade packages reuse the reference's top-level import names (`modeling`, `utils`,
 `layers`, `engine`), so reference code can never share an interpreter with them: the gpu parity tests and `bench.py` talk to
 the reference through this command-line program.
 

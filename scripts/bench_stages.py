@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Stage-level roofline numbers (HBM-bound kernels): CUDA-event timings over inputs larger than L2, algorithmic bytes
-from SURVEY 8(d).  Prints one JSON line; the summary lives in profiles/README.md."""
+from SURVEY 8(d).  Prints one JSON line."""
 import json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "st-nerf_b200"), os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden")):

@@ -24,7 +24,7 @@ namespace {
 struct SpaceNetDev {
   float* blob = nullptr;       // SIMT layout (transposed fp32)
   SpaceNetW w{};
-  TcNet tc{};                  // tcgen05 packing (mlp_tc.cu)
+  TcNet tc{};                  // tensor-core packing (mlp_tc.cu)
   bool loaded = false;
 };
 struct MotionNetDev {
@@ -71,7 +71,7 @@ struct stnerf_ctx {
   // Order of the split MMAs (mlp_tc.cu): 0 = interleaved everywhere, 1 = correction products first in the COARSE pass and in the
   // MotionNets (what the sample placement and the positions depend on), interleaved in the fine SpaceNet pass, 2 = first everywhere.
   // -1 (default): by precision -- STNERF_PREC_TC_3XF16_CF means 1, every other mode 0.
-  int lo_first_env = -1;       // STNERF_LO_FIRST=0|1|2 in the environment at create overrides (A/B: profiles/r02_ab_lo_first.json)
+  int lo_first_env = -1;       // STNERF_LO_FIRST=0|1|2 in the environment at create overrides (A/B experiments)
   int lo_first_mode() const { return lo_first_env >= 0 ? lo_first_env : (precision == STNERF_PREC_TC_3XF16_CF ? 1 : 0); }
   bool no_fuse = false;        // STNERF_NO_FUSE=1 in the environment at create: keep the coarse compositing in its own kernel (A/B)
   int* any_frac = nullptr;     // scratch flag for stnerf_motionnet(lerp_mode=-1)
@@ -164,7 +164,7 @@ const char* stnerf_strerror(int code) {
   switch (code) {
     case STNERF_OK: return "ok";
     case STNERF_EINVAL: return "invalid argument";
-    case STNERF_ENODEVICE: return "no usable CUDA device (needs sm_100)";
+    case STNERF_ENODEVICE: return "no usable CUDA device (needs sm_90)";
     case STNERF_ECUDA: return "CUDA runtime error (see stnerf_last_cuda_error)";
     case STNERF_ENOWEIGHTS: return "network weights not loaded";
     case STNERF_ENOMEM: return "out of device memory";
@@ -185,7 +185,7 @@ int stnerf_create(stnerf_handle* out, const stnerf_model_desc* d) {
   STNERF_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   STNERF_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (prop.major != 10) return STNERF_ENODEVICE;     // the cubin is sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return STNERF_ENODEVICE;     // the cubin is sm_90a only
   stnerf_ctx* c = new (std::nothrow) stnerf_ctx();
   if (!c) return STNERF_ENOMEM;
   c->desc = *d;
@@ -910,19 +910,9 @@ int stnerf_selftest_umma(float* max_err_host) {
   return tc_selftest(max_err_host);
 }
 
-int stnerf_selftest_umma_ts(float* max_err_host) {
-  if (!max_err_host) return STNERF_EINVAL;
-  return tc_selftest_ts(max_err_host);
-}
-
 int stnerf_selftest_umma_accum(int reps, float* max_err_host, float* mean_signed_rel_err_host) {
   if (!max_err_host || !mean_signed_rel_err_host || reps < 1 || reps > 4096) return STNERF_EINVAL;
   return tc_selftest_accum(reps, max_err_host, mean_signed_rel_err_host);
-}
-
-int stnerf_selftest_umma_pair(float* max_err_host) {
-  if (!max_err_host) return STNERF_EINVAL;
-  return tc_selftest_pair(max_err_host);
 }
 
 int stnerf_profile_begin(stnerf_handle c) {

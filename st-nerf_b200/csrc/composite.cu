@@ -428,6 +428,16 @@ __global__ void __launch_bounds__(256, 3) composite_pass_kernel(const CompositeA
   }
 }
 
+// SMs of the current device: the grids below are capped at a few waves of resident blocks
+static int device_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) {
+    cudaGetLastError();
+    return 1;
+  }
+  return n;
+}
+
 template <int NT, int NZ>
 static int launch_pass_t(const CompositeArgs& a, const DevScene& scene, int n_layers, const PassSmem& L, cudaStream_t st) {
   const size_t per_warp = (size_t)L.per_warp_floats * sizeof(float);
@@ -445,7 +455,8 @@ static int launch_pass_t(const CompositeArgs& a, const DevScene& scene, int n_la
   if (per_sm * wpb > 64) per_sm = 64 / wpb;
   if (per_sm < 1) per_sm = 1;
   long long blocks = (a.n + wpb - 1) / wpb;
-  if (blocks > 148LL * per_sm * 4) blocks = 148LL * per_sm * 4;
+  const long long cap = (long long)device_sms() * per_sm * 4;
+  if (blocks > cap) blocks = cap;
   kern<<<(int)blocks, wpb * 32, smem, st>>>(a, scene, n_layers, L);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
@@ -549,7 +560,7 @@ int launch_composite_simple(const float* t, const float* rgb, const float* sigma
   if (n <= 0) return STNERF_OK;
   const int block = 256;
   long long blocks = (n * 32 + block - 1) / block;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   composite_simple_kernel<<<(int)blocks, block, 0, st>>>(t, rgb, sigma, n, S, boarder, color, depth, acc, w);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
@@ -595,7 +606,7 @@ int launch_sample_pdf(const float* t, const float* w, const float* u, long long 
   if (smem > 48 * 1024)
     STNERF_CUDA(cudaFuncSetAttribute(sample_pdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   long long blocks = (n + wpb - 1) / wpb;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   sample_pdf_kernel<<<(int)blocks, wpb * 32, smem, st>>>(t, w, u, n, n1, n2, z, t_fine, per_warp);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;

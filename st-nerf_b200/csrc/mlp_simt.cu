@@ -1,7 +1,7 @@
 // fp32 CUDA-core (FFMA) evaluation of SpaceNet and MotionNet: precision mode STNERF_PREC_FP32_SIMT.
 //
 // This is the bit-closest mode (plain fp32 products, fp32 accumulation) and the on-device cross-check for the
-// tcgen05 kernels in mlp_tc.cu.  One persistent CTA per SM walks tiles of 64 points; activations live in
+// tensor-core kernels in mlp_tc.cu.  One persistent CTA per SM walks tiles of 64 points; activations live in
 // shared memory feature-major ([feature][point], padded) so the A operand of every layer is a broadcast
 // LDS.128 and the weights ([k][n], n contiguous) stream through L1 with fully coalesced 128 B rows.
 //

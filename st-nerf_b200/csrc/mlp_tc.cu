@@ -1,60 +1,34 @@
-// tcgen05 / TMEM evaluation of SpaceNet and MotionNet (precision modes TC_3XF16 "exact", TC_3XF16_CF "exact_cf", TC_MIXED "mixed",
-// TC_F16 "fast").
+// Hopper (sm_90a) tensor-core evaluation of SpaceNet and MotionNet with warpgroup MMAs (wgmma): precision modes TC_3XF16 "exact",
+// TC_3XF16_CF "exact_cf", TC_MIXED "mixed", TC_F16 "fast".
 //
-// Persistent CTAs (SpaceNet: one per SM; MotionNet: two per SM, see Sched<NET_MOTION>) walk tiles of 128 points.  Per tile the
-// whole network runs on-chip:
-//   * SpaceNet hidden activations (A operand) never leave TENSOR MEMORY (SPACE_A_TMEM, default): the epilogue converts a layer's
-//     fp32 accumulator columns IN PLACE into fp16 hi/lo pairs (tcgen05.ld -> bias -> ReLU -> split -> tcgen05.st: the 16 fp32
-//     columns of one K=16 step become 8 columns of hi pairs + 8 of lo pairs) and the next layer's MMAs read them from there
-//     (tcgen05.mma [d], [a], b-desc) while accumulating into the other buffer -- the two 128x256 buffers alternate between
-//     "accumulator" and "A operand", shared memory only holds the input encoding and the weight ring;
-//   * MotionNet (and the SPACE_A_TMEM=0 / CTA-pair builds) keep the activations in shared memory as fp16 hi/lo pairs in the
-//     canonical 128B-swizzled K-major UMMA layout ([128 rows x 64 k] blocks); the encoding always lives there;
-//   * weights (B operand) are pre-packed on the host into [N out-rows x 32 k] fp16 blocks (N = 256 or 128) that are
-//     already the 64B-swizzled shared-memory image, in the exact order the MMA warp consumes them, and stream through
-//     a ring of 16 KB stages (SpaceNet: 8; MotionNet: 4 x 8 KB) with 1-D bulk async copies (cp.async.bulk + mbarrier complete_tx) from L2;
-//   * every MMA is M=128 x N=256 (or 128) x K=16;
-//   * accumulators live in TMEM (two 128x256 fp32 buffers = all 512 columns) so the epilogue of layer k
-//     (tcgen05.ld -> bias -> ReLU -> fp16 hi/lo split -> store) overlaps the MMAs of layer k+1; the hand-off is per 32-k
-//     SUB-chunk and per HALF (a_ready[2c + sub]: the fp16 hi parts, a_ready[8 + 2c + sub]: the lo parts; an epilogue thread owns
-//     16 columns of each half of a 64-column chunk): the next layer opens with Ahi*Wlo off the lo weight stage, which needs the hi
-//     parts only, so its first MMAs wait for a TMEM load + 16 columns of bias / ReLU / conversion, not for a whole chunk;
+// Persistent CTAs (one per SM) walk tiles of 128 points.  Per tile the whole network runs on-chip:
+//   * CTA = three warpgroups.  Warpgroup 0: warp 0 streams the weights, warps 2..3 are the coarse-pass compositing warps
+//     (FuseCoarse, below).  Warpgroups 1 and 2 are the math warpgroups: warpgroup 1 + w owns rows 64 w .. 64 w + 63 of the tile,
+//     issues their MMAs (wgmma m64 x N x k16, N = 256 or 128, accumulators in registers) and runs their epilogues.  The two
+//     math warpgroups share nothing but the weight ring, so while one runs its epilogue the other keeps the tensor cores busy;
+//   * activations (A operand) live in shared memory as fp16 hi/lo pairs in the canonical 128B-swizzled K-major layout
+//     ([128 rows x 64 k] blocks); a layer's epilogue overwrites the rows its own MMAs have just finished reading;
+//   * weights (B operand) are pre-packed on the host into [N out-rows x 32 k] fp16 blocks that are already the 64B-swizzled
+//     shared-memory image, in the exact order the math warpgroups consume them, and stream through a ring of stages with 1-D
+//     bulk async copies (cp.async.bulk + mbarrier complete_tx) from L2; a slot is refilled once every math warp has seen the
+//     MMAs that read it retire (wgmma.wait_group);
 //   * exact mode issues three fp16 MMAs per product, D += Ahi*Whi + Alo*Whi + Ahi*Wlo (fp32 accumulate), which reproduces fp32
 //     products to ~2^-22 (SURVEY App. C.3: the only tensor-core formulation inside the 1e-3 gate); mixed mode keeps that
 //     everywhere the density depends on and runs the colour-only layer rgb_net.1 in one pass;
 //   * order of the three products (template parameter LOFIRST): interleaved per 32-k sub-chunk (default: every weight stage is
 //     streamed once), or -- TC_3XF16_CF "exact_cf", coarse pass + MotionNets -- the two correction products FIRST over the whole K
-//     range, then Ahi*Whi.  The tensor core truncates when it adds into its fp32 accumulator (stnerf_selftest_umma_accum), an
-//     error relative to the accumulator's magnitude at that moment; corrections-first truncates at full magnitude K/16 instead
-//     of 3K/16 times per layer (sigma error 7e-6 -> 2e-6 rel. rms) and streams the hi weight stages twice (+2.5 % per step);
-//   * the input encoding of tile i+1 is written while the tensor core works on the late layers of tile i;
+//     range, then Ahi*Whi, so the accumulator is small while the corrections are added (stnerf_selftest_umma_accum measures how
+//     the tensor core rounds its fp32 accumulation); the hi weight stages are then streamed twice;
 //   * relu(PE(dir) | PE(time)) enters rgb_net.1 as a per-ray fp32 bias computed by head_bias_kernel
 //     (b1 + W1[:,256:] . relu(enc)), so the last GEMM is a clean K=256;
-//   * the 1-wide density head, the 3-wide rgb / flow heads and all biases are fp32 FFMA work in the epilogue.
-//
-//   * SpaceNet CTAs run as 2-CTA clusters that share the weight stream: each CTA pulls half of every stage from L2 and multicasts
-//     it into both shared memories (SPACE_WSHARE); tiles, accumulators and MMAs stay per CTA;
-//   * in the coarse pass (n1 = 64: a tile = two whole rays of one layer) two otherwise idle warps composite the tile's rgb / sigma
+//   * the 1-wide density head, the 3-wide rgb / flow heads and all biases are fp32 FFMA work in the epilogue;
+//   * in the coarse pass (n1 = 64: a tile = two whole rays of one layer) the two compositing warps composite the tile's rgb / sigma
 //     rows and draw + merge the fine depths (FuseCoarse, resample.cuh): the coarse samples never leave the SM.
-//
-// The producer and the MMA issuer run their loops WARP-WIDE and hand every weight stage to one asm block in which elect.sync picks
-// the issuing lane (issue_stage / load_stage_elect): inside a plain `if (lane == 0)` ptxas wraps each tcgen05 / bulk-copy
-// instruction in an elect-execute-retire loop and the single issuing thread ends up on the critical path (-4.9 % per step).
-//
-// Warp roles (SpaceNet, 384 threads): warp 0 = weight producer, warp 1 = MMA issuer + TMEM owner, warps 2..3 = compositing warps
-// (coarse-pass fusion), warps 4..11 = epilogue / encoding warps: warp%4 selects the TMEM lane quarter (row = 32*(warp%4) + lane),
-// (warp-4)/4 the column half of every 64-column chunk and the half of the encoding frequencies the thread computes for its row.
-// (MotionNet, 320 threads: the same roles without warps 2..3, epilogue warps 2..9.)
-//
-// Build flags: SPACE_A_TMEM=0 keeps the SpaceNet activations in shared memory (A/B reference: bit-identical results, same speed --
-// the kernel is bound by the power cap, not by the shared-memory port: profiles/r02_ab_a_in_tmem.json), SPACE_RING the depth of
-// the SpaceNet weight ring under SPACE_A_TMEM (8; the shared-memory build has room for 4); SPACE_WSHARE=0 switches the shared weight stream off (every CTA then pulls all 1.8 MB per tile from L2 itself);
-// SPACE_CTA_PAIR=1 runs the SpaceNet tiles as 2-CTA clusters on one cta_group::2 accumulator (correct, not faster: DESIGN.md 8);
-// MOTION_CTAS_PER_SM=1 restores the single-CTA MotionNet layout, PRODUCER_ELECT=0 the single-lane weight producer,
-// SPACE_ENC_FIRST=0 the skip layer's original chunk order (A/B references).
 //
 // Restates modeling/spacenet.py:101-160, modeling/motion_net.py:34-71, utils/dimension_kernel.py:24-33.
 #include <cuda_fp16.h>
+#include <string.h>
+#include <type_traits>
 #include <vector>
 #include "mlp_tc.cuh"
 #include "resample.cuh"
@@ -63,53 +37,18 @@ namespace stnerf {
 
 namespace {
 
-#ifndef SPACE_CTA_PAIR
-#define SPACE_CTA_PAIR 0              // 1: SpaceNet tiles run as CTA pairs sharing one cta_group::2 accumulator (see mlp_tc_kernel)
-#endif
-#ifndef SPACE_WSHARE
-#define SPACE_WSHARE 1                // 1 (default): SpaceNet CTAs run as 2-CTA clusters that SHARE THE WEIGHT STREAM: each CTA pulls half of
-#endif                                //    every stage from L2 and multicasts it into both shared memories (MMAs stay per CTA, cta_group::1);
-                                      //    0: every CTA streams all weights itself (A/B reference)
-#ifndef SPACE_A_TMEM
-#define SPACE_A_TMEM 1                // 1 (default): the SpaceNet hidden activations never leave TENSOR MEMORY: the epilogue converts a layer's
-#endif                                //    fp32 accumulator columns IN PLACE into the fp16 hi/lo A operand of the next layer (tcgen05.st) and
-                                      //    the MMAs read A from tensor memory (tcgen05.mma [d], [a], b-desc); 0: A through shared memory (A/B)
-#ifndef SPACE_RING
-#define SPACE_RING 8                  // weight-ring depth of the SpaceNet kernel under SPACE_A_TMEM (16 KB stages; the activations' 128 KB are free)
-#endif
-#ifndef SPACE_ENC_FIRST
-#define SPACE_ENC_FIRST 1             // 1 (default): the SpaceNet skip layer consumes its encoding chunk first (Sched::enc_first; 0: last, A/B)
-#endif
-#ifndef PRODUCER_ELECT
-#define PRODUCER_ELECT 1              // 1 (default): the weight producer runs warp-wide with one elected issuing lane (0: single lane, A/B)
-#endif
-#ifndef MOTION_CTAS_PER_SM
-#define MOTION_CTAS_PER_SM 2          // resident CTAs per SM of the MotionNet instantiation (1 = single-CTA layout, kept for A/B)
-#endif
 constexpr int TILE_M = 128;
 constexpr int ABLOCK = 16384;                // activation block [128 rows x 64 k] fp16, SWIZZLE_128B
 constexpr int STAGE_BYTES = 16384;           // weight stage   [256 rows x 32 k] fp16, SWIZZLE_64B (N=128 layers use half)
-constexpr int NSTAGE = 4;
-constexpr int NTHREADS = 384;
-constexpr int EPI_WARP0 = 4, N_EPI_WARPS = 8;
-
-// shared memory map (bytes, from a 1024-aligned base)
-constexpr int SM_ACT = 0;                    // 8 blocks
-constexpr int SM_ENC = 8 * ABLOCK;           // 2 blocks: hi, lo (SpaceNet).  MotionNet: ACT = blocks 0-3, ENC = blocks 4-7
-constexpr int SM_RING = 10 * ABLOCK;
-constexpr int SM_MISC = SM_RING + NSTAGE * STAGE_BYTES;
-constexpr int MAX_STAGE = 8;                 // ring slots a kernel may use (CTA-pair mode: 8 half-size stages in the same 64 KB)
-constexpr int BAR_WFULL = 0, BAR_WEMPTY = 8, BAR_WPEER = 16, BAR_AREADY = 24, BAR_DFULL = 41, BAR_DEMPTY = 43,
-              BAR_RAWFULL = 45, BAR_RAWEMPTY = 46;                                                                // 47 barriers
-// a_ready[2c + sub]: the fp16 HI half of 32-k sub-chunk `sub` of activation chunk c is written; [8 + 2c + sub]: its LO half;
-// [16]: the tile's encoding (hi and lo)
-constexpr int N_AREADY = 17, AREADY_LO = 8, AREADY_ENC = 16;
-constexpr int MISC_TMEM = 376;
-constexpr int MISC_PART = 384;               // float[128][4]: head partial sums of column-half 1; with the coarse-pass fusion: the
-                                             // tile's final (rgb logits, sigma) rows, read by the compositing warps
+constexpr int NTHREADS = 384;                // warpgroup 0: producer + compositing warps; warpgroups 1, 2: math
+constexpr int MATH_WG0 = 1, N_MATH_WARPS = 8;
+constexpr int MAX_STAGE = 8;
+constexpr int BAR_WFULL = 0, BAR_WEMPTY = 8, BAR_RAWFULL = 16, BAR_RAWEMPTY = 18;          // 20 barriers
+// misc region: barriers | per-row point info of the current tile | final rows for the compositing warps | their scratch
+constexpr int MISC_ROWS = 256;               // Pt[128]
+constexpr int MISC_PART = MISC_ROWS + 128 * 24;   // float4[128]: the tile's final (rgb logits, sigma) rows (coarse-pass fusion)
 constexpr int MISC_CDF = MISC_PART + 2048;   // fused compositing warps: cdf / depth scratch, 2 x 64 floats
-constexpr int SM_TOTAL = SM_MISC + MISC_CDF + 512;
-static_assert(SM_TOTAL <= 232448, "shared memory budget (227 KB per CTA)");
+constexpr int MISC_TOTAL = MISC_CDF + 512;
 
 // ---------------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -122,253 +61,129 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar), "r"((uint32_t)pred)
+               : "memory");
+}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Bounded wait: a protocol bug traps (the kernel aborts with an error) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (the kernel aborts with an error) instead of hanging the GPU.  The loop lives inside one asm
+// block so that the compiler sees no divergent branch in front of the warpgroup MMAs that follow a wait.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin) {
-    if (spin > (1u << 26)) __trap();
-  }
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .u32 c;\n\t"
+      "mov.u32 c, 0;\n"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra.uni DONE_%=;\n\t"
+      "add.u32 c, c, 1;\n\t"
+      "setp.gt.u32 p, c, 67108864;\n\t"
+      "@p trap;\n\t"
+      "bra.uni WAIT_%=;\n"
+      "DONE_%=:\n\t}" ::"r"(bar), "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-// Multicast forms for the shared weight stream (SPACE_WSHARE): the copy lands at the same shared-memory offset of every CTA in
-// `mask` and completes bytes on the mbarrier at the same offset there; the commit arrives on that barrier in every CTA of `mask`.
-__device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// A operand in tensor memory ([128 lanes x 8 columns] of fp16 pairs at a_tmem), B through its shared-memory descriptor
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// ---- warp-wide issue helpers: the MMA warp runs its loop on all 32 lanes, ONE elected lane issues ------------------------------
-// Under a plain `if (lane == 0)` ptxas cannot know that a single thread is active: it wraps every tcgen05 instruction in an
-// "elect an active lane, execute, retire it, repeat" loop and rebuilds both 64-bit descriptors per MMA.  The issuing thread is
-// latency-critical (a few extra instructions per MMA were measured at -4 %, profiles/r02_ab_lo_first.json).  Here the lane is
-// chosen by elect.sync inside the asm block (predicated instructions, no loop), a whole weight stage is issued per block and a
-// descriptor is a precomputed low word + a constant high word (32 bytes along K = +2 in the 16-byte address field).
-constexpr uint32_t DESC_HI_SW128 = (1024u >> 4) | (1u << 14) | (2u << 29);      // SBO 1024 B, version 1, SWIZZLE_128B
-constexpr uint32_t DESC_HI_SW64 = (512u >> 4) | (1u << 14) | (4u << 29);        // SBO 512 B, version 1, SWIZZLE_64B
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3FFFu) | (1u << 16); }
+// named barrier of one math warpgroup (ids 1, 2; id 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// operands: %0 accumulator (TMEM), %1 A block 0, %2 A block 1, %3 weight stage, %4 instruction descriptor, %5 accumulate flag of the
-// first MMA, %6 barrier to commit to, %7 / %8 descriptor high words (A / B), %9 multicast mask
-#define STNERF_ISSUE_HEAD                                                                                                  \
-  "{\n\t.reg .pred pe, pa, pt;\n\t.reg .b64 da, db0, db1;\n\t.reg .b32 t;\n\t"                                             \
-  "elect.sync _|pe, 0xffffffff;\n\t"                                                                                       \
-  "setp.ne.b32 pa, %5, 0;\n\t"                                                                                             \
-  "setp.eq.b32 pt, %5, %5;\n\t"                                                                                            \
-  "mov.b64 db0, {%3, %8};\n\t"                                                                                             \
-  "add.u32 t, %3, 2;\n\t"                                                                                                  \
-  "mov.b64 db1, {t, %8};\n\t"
-#define STNERF_ISSUE_A(AREG, PFIRST)                                                                                       \
-  "mov.b64 da, {" AREG ", %7};\n\t"                                                                                        \
-  "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], da, db0, %4, " PFIRST ";\n\t"                                              \
-  "add.u32 t, " AREG ", 2;\n\t"                                                                                            \
-  "mov.b64 da, {t, %7};\n\t"                                                                                               \
-  "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], da, db1, %4, pt;\n\t"
-#define STNERF_ISSUE_COMMIT_MC "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%6], %9;\n\t}"
-#define STNERF_ISSUE_COMMIT_1 "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%6];\n\t}"
-#define STNERF_ISSUE_OPERANDS                                                                                              \
-  ::"r"(d_tmem), "r"(a0), "r"(a1), "r"(w), "r"(idesc), "r"(acc0), "r"(bar), "r"(DESC_HI_SW128), "r"(DESC_HI_SW64), "h"(mask) : "memory"
-
-// One weight stage [N x 32 k] (descriptor word `w`) times the 32-k slice of the A block at `a0` (two K=16 MMAs) and, with NA == 2,
-// of a second A block at `a1` as well (four MMAs), then tcgen05.commit on `bar` (MC: in both CTAs of the cluster).
-// acc0 == 0: the first MMA overwrites the accumulator.  Executed by the whole, converged warp.
-template <int NA, bool MC>
-__device__ __forceinline__ void issue_stage(uint32_t d_tmem, uint32_t a0, uint32_t a1, uint32_t w, uint32_t idesc, uint32_t acc0,
-                                            uint32_t bar) {
-  const uint16_t mask = 3;
-  if (NA == 1 && MC) asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A("%1", "pa") STNERF_ISSUE_COMMIT_MC STNERF_ISSUE_OPERANDS);
-  if (NA == 1 && !MC) asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A("%1", "pa") STNERF_ISSUE_COMMIT_1 STNERF_ISSUE_OPERANDS);
-  if (NA == 2 && MC)
-    asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A("%1", "pa") STNERF_ISSUE_A("%2", "pt") STNERF_ISSUE_COMMIT_MC STNERF_ISSUE_OPERANDS);
-  if (NA == 2 && !MC)
-    asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A("%1", "pa") STNERF_ISSUE_A("%2", "pt") STNERF_ISSUE_COMMIT_1 STNERF_ISSUE_OPERANDS);
-}
-// The same with the A operand in TENSOR memory (SPACE_A_TMEM): a0 / a1 are tensor-memory addresses of [128 lanes x 8 columns] fp16x2
-// slices (row = lane, column c = k elements 2c, 2c+1); the second K=16 step of the stage sits 16 columns further (8 hi + 8 lo columns
-// per 16 k, see epi_hidden_chunk).
-#define STNERF_ISSUE_A_TS(AREG, PFIRST)                                                                                    \
-  "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [" AREG "], db0, %4, " PFIRST ";\n\t"                                      \
-  "add.u32 t, " AREG ", 16;\n\t"                                                                                           \
-  "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [t], db1, %4, pt;\n\t"
-template <int NA, bool MC>
-__device__ __forceinline__ void issue_stage_ts(uint32_t d_tmem, uint32_t a0, uint32_t a1, uint32_t w, uint32_t idesc, uint32_t acc0,
-                                               uint32_t bar) {
-  const uint16_t mask = 3;
-  if (NA == 1 && MC) asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A_TS("%1", "pa") STNERF_ISSUE_COMMIT_MC STNERF_ISSUE_OPERANDS);
-  if (NA == 1 && !MC) asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A_TS("%1", "pa") STNERF_ISSUE_COMMIT_1 STNERF_ISSUE_OPERANDS);
-  if (NA == 2 && MC)
-    asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A_TS("%1", "pa") STNERF_ISSUE_A_TS("%2", "pt") STNERF_ISSUE_COMMIT_MC STNERF_ISSUE_OPERANDS);
-  if (NA == 2 && !MC)
-    asm volatile(STNERF_ISSUE_HEAD STNERF_ISSUE_A_TS("%1", "pa") STNERF_ISSUE_A_TS("%2", "pt") STNERF_ISSUE_COMMIT_1 STNERF_ISSUE_OPERANDS);
-}
-// eight 32-bit columns of this thread's lane (row) -> tensor memory; the wait makes the warp's stores visible to later tcgen05 ops
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// tcgen05.commit by one elected lane of the converged warp ("every MMA issued so far has retired" -> one arrival on `bar`)
-__device__ __forceinline__ void commit_elect(uint32_t bar) {
+// Weight-stage load by one elected lane of the converged producer warp: announce the bytes on `bar`, then the bulk copy.
+__device__ __forceinline__ void load_stage_elect(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile(
       "{\n\t.reg .pred pe;\n\t"
       "elect.sync _|pe, 0xffffffff;\n\t"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
+      "@pe mbarrier.arrive.expect_tx.shared::cta.b64 _, [%3], %2;\n\t"
+      "@pe cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}" ::"r"(dst),
+      "l"(src), "r"(bytes), "r"(bar)
       : "memory");
 }
 
-// Weight-stage load by one elected lane of the converged producer warp: announce `expect` bytes on `bar`, then the bulk copy
-// (MC: multicast into both CTAs of the cluster, completing bytes on the barrier at the same offset in each).
-template <bool MC>
-__device__ __forceinline__ void load_stage_elect(uint32_t dst, const void* src, uint32_t copy_bytes, uint32_t expect, uint32_t bar) {
-  const uint16_t mask = 3;
-  if (MC)
-    asm volatile(
-        "{\n\t.reg .pred pe;\n\t"
-        "elect.sync _|pe, 0xffffffff;\n\t"
-        "@pe mbarrier.arrive.expect_tx.shared::cta.b64 _, [%3], %4;\n\t"
-        "@pe cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %5;\n\t}" ::"r"(dst),
-        "l"(src), "r"(copy_bytes), "r"(bar), "r"(expect), "h"(mask)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred pe;\n\t"
-        "elect.sync _|pe, 0xffffffff;\n\t"
-        "@pe mbarrier.arrive.expect_tx.shared::cta.b64 _, [%3], %4;\n\t"
-        "@pe cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}" ::"r"(dst),
-        "l"(src), "r"(copy_bytes), "r"(bar), "r"(expect)
-        : "memory");
+// ---- warpgroup MMA ----------------------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptors (sm_90 layout), K-major operands: start address >> 4 in bits 0-13, leading byte offset
+// (unused by swizzled K-major operands) in 16-29, stride byte offset (8-row groups) >> 4 in 32-45, swizzle mode in 62-63.
+//   A: SWIZZLE_128B (mode 1), 8-row groups 1024 B apart;  B: SWIZZLE_64B (mode 2), 8-row groups 512 B apart.
+// One K=16 step further along K is +32 bytes on the start address (the swizzle is applied to the absolute address).
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ uint64_t desc_sw64(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across a wgmma.wait_group
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 256] += A[64 x 16] * B[256 x 16]^T, both K-major in shared memory; fp16 in, fp32 accumulate in registers
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(1));
 }
-// two 16-column loads (the epilogue's two passes over a 64-column chunk) behind one wait
-__device__ __forceinline__ void tmem_ld16x2_issue(uint32_t taddr0, uint32_t taddr1, uint32_t (&r)[32]) {
+// D[64 x 128] += A[64 x 16] * B[128 x 16]^T, both K-major in shared memory; fp16 in, fp32 accumulate in registers
+__device__ __forceinline__ void wgmma_n128(float (&d)[128], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr0)
-      : "memory");
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr1)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(1));
 }
-// The registers are threaded through the wait so no consumer can be scheduled ahead of it.
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// ---- CTA-pair (cta_group::2) variants: the two CTAs of a cluster issue ONE MMA of M = 256 from the leader; each CTA keeps its
-// own 128 rows of A and half of the B rows in its shared memory, and its 128 accumulator rows in its tensor memory.
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t map_to_cta(uint32_t local_saddr, uint32_t rank) {     // shared::cluster address of a peer's copy
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_saddr), "r"(rank));
-  return r;
-}
-// Remote arrive / wait with the DEFAULT semantics (release / acquire at CTA scope), as cutlass::arch::ClusterBarrier does.
-// Asking for `.release.cluster` / `.acquire.cluster` makes ptxas emit MEMBAR.ALL.GPU before every arrive and CCTL.IVALL (a full
-// L1 invalidate) after every successful wait -- measured 1.7x slower on the whole kernel.  What crosses the CTA boundary here is
-// shared memory written through `fence.proxy.async` and tensor memory ordered by tcgen05 fences, neither of which lives in L1.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) { mbar_wait(bar, parity); }
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {       // arrives on the barrier at this offset in BOTH CTAs
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(mask)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_k16(float (&d)[128], uint64_t da, uint64_t db) {
+  if (N == 256) wgmma_n256(d, da, db);
+  else wgmma_n128(d, da, db);
 }
 
 // {lo16 = fp16(a), hi16 = fp16(b)}, saturating to +-65504 (fp16 range guard of the split)
@@ -380,20 +195,6 @@ __device__ __forceinline__ uint32_t pack_f16x2(float a, float b) {
 __device__ __forceinline__ float2 unpack_f16x2(uint32_t p) {
   return __half22float2(*reinterpret_cast<const __half2*>(&p));
 }
-
-// UMMA shared-memory descriptors (cute::UMMA::SmemDescriptor bit layout), K-major operands.
-//   A: SWIZZLE_128B, 8-row groups 1024 B apart;  B: SWIZZLE_64B, 8-row groups 512 B apart.
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)4 << 61);
-}
-// Instruction descriptor: fp16 A/B (K-major), fp32 D, M = 128 (cute::UMMA::InstrDescriptor).
-__host__ __device__ constexpr uint32_t idesc_n(uint32_t n) { return (1u << 4) | ((n >> 3) << 17) | ((128u >> 4) << 24); }
-__host__ __device__ constexpr uint32_t idesc_pair_n(uint32_t n) { return (1u << 4) | ((n >> 3) << 17) | ((256u >> 4) << 24); }   // M = 256 over a CTA pair
 
 // byte offset of element (row, col) of a [rows x 64] fp16 block, 128B-swizzled K-major (activations)
 __host__ __device__ inline uint32_t sw128_offset(int row, int col) {
@@ -412,64 +213,33 @@ enum { NET_SPACE = 0, NET_MOTION = 1 };
 template <int NET> struct Sched;
 template <> struct Sched<NET_SPACE> {
   static constexpr int N_LAYERS = 8;
-#if SPACE_A_TMEM && !SPACE_CTA_PAIR
-  // hidden activations in tensor memory: shared memory holds the encoding (2 blocks), a 4 KB scratch (head half sums) and a
-  // SPACE_RING-deep weight ring
-  static constexpr int act_base = 0, enc_base = 0, scratch_base = 2 * ABLOCK;
-  static constexpr int n_stage = SPACE_RING;
-  static constexpr int ring_base = 2 * ABLOCK + 4096, stage_bytes = STAGE_BYTES, misc_base = ring_base + n_stage * STAGE_BYTES,
-                       smem_total = misc_base + MISC_CDF + 512;
-  static_assert(n_stage <= MAX_STAGE && smem_total <= 232448, "SpaceNet ring");
-#else
-  static constexpr int act_base = SM_ACT, enc_base = SM_ENC, scratch_base = SM_ACT;
-  static constexpr int n_stage = NSTAGE;
-  static constexpr int ring_base = SM_RING, stage_bytes = STAGE_BYTES, misc_base = SM_MISC, smem_total = SM_TOTAL;
-#endif
+  // shared memory: activations (4 hi + 4 lo blocks), encoding (hi, lo), a 3-deep ring of 16 KB weight stages, misc
+  static constexpr int act_base = 0, enc_base = 8 * ABLOCK;
   static constexpr int LO_STRIDE = 4 * ABLOCK;          // ACT lo blocks follow the 4 hi blocks
   static constexpr int ENC_LO_STRIDE = ABLOCK;
-  static constexpr int ENC_LAST_USE = 4;                // last layer whose MMAs read the encoding buffer
+  static constexpr int n_stage = 3, stage_bytes = STAGE_BYTES;
+  static constexpr int ring_base = 10 * ABLOCK, misc_base = ring_base + n_stage * stage_bytes, smem_total = misc_base + MISC_TOTAL;
+  static_assert(smem_total <= 232448, "shared memory budget (227 KB per CTA)");
   __host__ __device__ static constexpr int n_out(int l) { return l == 7 ? 128 : 256; }
   __host__ __device__ static constexpr int act_chunks(int l) { return l == 0 ? 0 : 4; }
   __host__ __device__ static constexpr int enc_chunks(int l) { return (l == 0 || l == 4) ? 1 : 0; }
-  // the skip layer consumes its encoding chunk FIRST: those MMAs do not depend on the previous layer's epilogue, so they run
-  // while the tensor pipe would otherwise wait for the first activation sub-chunk (the weight stream is packed in the same order)
-  __host__ __device__ static constexpr bool enc_first(int l) { return SPACE_ENC_FIRST != 0 && l == 4; }
-  // CTA shape and shared/tensor-memory map: one CTA per SM, the whole 227 KB and all 512 TMEM columns
-  static constexpr int N_THREADS = NTHREADS, EPI_W0 = EPI_WARP0, CTAS_PER_SM = 1;
-  static constexpr int tmem_cols = 512, d_stride = 256;
-  static constexpr bool ENC_ALIASES_ACT = false;
+  // the skip layer consumes its encoding chunk FIRST (the weight stream is packed in the same order)
+  __host__ __device__ static constexpr bool enc_first(int l) { return l == 4; }
 };
 template <> struct Sched<NET_MOTION> {
-  static constexpr int n_stage = NSTAGE;
   static constexpr int N_LAYERS = 5;
+  // the encoding (read by layer 0 only) shares the activation blocks: layer 0's epilogue overwrites it after its MMAs retired
+  static constexpr int act_base = 0, enc_base = 0;
   static constexpr int LO_STRIDE = 2 * ABLOCK;
   static constexpr int ENC_LO_STRIDE = 2 * ABLOCK;
-  static constexpr int ENC_LAST_USE = 0;
+  static constexpr int n_stage = 8, stage_bytes = 8192;
+  static constexpr int ring_base = 4 * ABLOCK, misc_base = ring_base + n_stage * stage_bytes, smem_total = misc_base + MISC_TOTAL;
   __host__ __device__ static constexpr int n_out(int) { return 128; }
   __host__ __device__ static constexpr int act_chunks(int l) { return l == 0 ? 0 : 2; }
   __host__ __device__ static constexpr int enc_chunks(int l) { return l == 0 ? 2 : 0; }
   __host__ __device__ static constexpr bool enc_first(int) { return false; }
-#if MOTION_CTAS_PER_SM == 2
-  // Two CTAs per SM.  A MotionNet tile is a serial chain (5 layers of N=128: two 64-column chunks per layer leave nothing to
-  // pipeline inside a tile), so the tensor pipe idles while the epilogue warps work and vice versa; a second resident CTA
-  // fills those gaps.  Budget per CTA: 100 KB of shared memory (the encoding shares the activation blocks -- it is
-  // written after the last layer's MMAs have retired -- and the N=128 weight stages are 8 KB), 256 TMEM columns
-  // (2 x 128 accumulators), 10 warps (no spare warps) so that 2 x 320 threads leave 96 registers per thread.
-  static constexpr int act_base = SM_ACT, enc_base = SM_ACT, scratch_base = SM_ACT;
-  static constexpr int N_THREADS = 320, EPI_W0 = 2, CTAS_PER_SM = 2;
-  static constexpr int ring_base = 4 * ABLOCK, stage_bytes = 8192, misc_base = ring_base + NSTAGE * stage_bytes,
-                       smem_total = misc_base + MISC_CDF;
-  static constexpr int tmem_cols = 256, d_stride = 128;
-  static constexpr bool ENC_ALIASES_ACT = true;
-#else
-  static constexpr int act_base = SM_ACT, enc_base = SM_ACT + 4 * ABLOCK, scratch_base = SM_ACT;
-  static constexpr int N_THREADS = NTHREADS, EPI_W0 = EPI_WARP0, CTAS_PER_SM = 1;
-  static constexpr int ring_base = SM_RING, stage_bytes = STAGE_BYTES, misc_base = SM_MISC, smem_total = SM_TOTAL;
-  static constexpr int tmem_cols = 512, d_stride = 256;
-  static constexpr bool ENC_ALIASES_ACT = false;
-#endif
 };
-static_assert(2 * (Sched<NET_MOTION>::smem_total + 1024) <= 233472 || Sched<NET_MOTION>::CTAS_PER_SM == 1, "two MotionNet CTAs per SM");
+static_assert(Sched<NET_SPACE>::n_stage <= MAX_STAGE && Sched<NET_MOTION>::n_stage <= MAX_STAGE, "barrier slots");
 
 template <int NET>
 __host__ __device__ constexpr size_t stream_bytes_per_tile() {
@@ -481,17 +251,15 @@ __host__ __device__ constexpr size_t stream_bytes_per_tile() {
 }
 
 struct TcParams {
-  FuseCoarse fuse;            // SpaceNet, coarse pass: per-layer compositing + resampling in the kernel's spare warps
+  FuseCoarse fuse;            // SpaceNet, coarse pass: per-layer compositing + resampling in the compositing warps
   PointSrc src;
   const uint8_t* wstream;     // packed weight stream (hi/lo stages in consumption order)
   const float* aux;           // fp32: biases [8][256] | w_sigma[256] | b_sigma | w_out[3][128] | b_out[3]
   const float* cbuf;          // SpaceNet: per-slot rgb_net.1 bias (b1 + W1[:,256:].relu(enc(dir,time))), [slots][128]
   int exact;                  // 1: 3-term split, 0: single fp16 pass
   int single_last;            // with exact: the LAST GEMM layer (SpaceNet rgb_net.1, colour branch only) runs a single pass
-  int lo_first;               // split layers (selects the kernel instantiation): 0 = interleaved per 32-k sub-chunk (default: hi stages
-                              // streamed once); 1 = correction products first over the whole K range, then Ahi*Whi (fewer truncations
-                              // at full magnitude, sigma error / 3; hi weight stages streamed twice: measured -7 % when used in the
-                              // coarse pass + MotionNets only)
+  int lo_first;               // split layers (selects the kernel instantiation): 0 = interleaved per 32-k sub-chunk (hi stages
+                              // streamed once); 1 = correction products first over the whole K range, then Ahi*Whi
   // outputs
   float* raw;                 // float4 per sample (pipeline mode)
   float* rgb_out;             // explicit mode
@@ -504,6 +272,7 @@ struct TcParams {
 
 constexpr int AUX_BIAS = 0, AUX_WSIG = 8 * 256, AUX_BSIG = AUX_WSIG + 256, AUX_WOUT = AUX_BSIG + 4,
               AUX_BOUT = AUX_WOUT + 3 * 128, AUX_FLOATS = AUX_BOUT + 4;
+
 
 // ---------------------------------------------------------------------------------------------------------
 // point fetch (same arithmetic as mlp_simt.cu::fetch_point)
@@ -681,124 +450,6 @@ __device__ __forceinline__ void encode_piece(uint8_t* smem, const Pt& pt, int ro
   }
 }
 
-#ifdef STNERF_TIMING
-struct EpiTiming { long long ld = 0, math = 0, fence = 0, arrive = 0, wait_dfull = 0, n = 0, enc = 0, last_wait = 0, last_epi = 0, tiles = 0; };
-#define TSTAMP(x) const long long x = clock64()
-#else
-#define TSTAMP(x)
-#endif
-
-template <bool SIGMA, bool PAIR = false, bool ATMEM = false>
-__device__ __forceinline__ float epi_hidden_chunk(uint32_t dcol, int j, int hh, int row, const float* __restrict__ bias,
-                                                  const float* __restrict__ wdot, uint8_t* blk, int lo_stride, bool exact,
-                                                  int lane, uint32_t ready_bar, float dot
-#ifdef STNERF_TIMING
-                                                  , EpiTiming& tm
-#endif
-) {
-  // The thread owns columns [hh*16, hh*16+16) of BOTH 32-column halves of the chunk.  Per half ("pass"): the fp16 HI parts of its
-  // 16 columns are stored and announced first (ready_bar + 8*pass: all eight warps arrive), the LO parts and -- layer 6 -- the
-  // density dot product afterwards (ready_bar + 8*(AREADY_LO + pass)).  The next layer's first MMAs (Ahi x Wlo, then Ahi x Whi)
-  // need only the HI half of the first sub-chunk, so the per-layer bubble the tensor pipe waits out is a TMEM load + 16 columns of
-  // bias / ReLU / fp16 conversion + one proxy fence; the LO half is due four MMAs later.
-  // ATMEM: the operand goes back into TENSOR memory, in place of the fp32 columns it was computed from -- the thread's 16 accumulator
-  // columns [c0, c0+16) of a pass become 8 columns of packed HI pairs [c0, c0+8) and 8 of LO pairs [c0+8, c0+16): one K=16 step of
-  // the next layer's A operand (k = c0 .. c0+15; column e holds k = c0+2e in its low half, c0+2e+1 in its high half).
-  uint32_t acc[32];
-  const int colA = j * 64 + hh * 16, colB = colA + 32;
-  TSTAMP(t0);
-  tmem_ld16x2_issue(dcol + (uint32_t)colA, dcol + (uint32_t)colB, acc);
-  float4 bv[8], wv[8];
-  {
-    const float4* bpA = reinterpret_cast<const float4*>(bias + colA);     // L1-resident; overlaps the TMEM load
-    const float4* bpB = reinterpret_cast<const float4*>(bias + colB);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { bv[i] = __ldg(bpA + i); bv[4 + i] = __ldg(bpB + i); }
-    if (SIGMA) {
-      const float4* wpA = reinterpret_cast<const float4*>(wdot + colA);
-      const float4* wpB = reinterpret_cast<const float4*>(wdot + colB);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { wv[i] = __ldg(wpA + i); wv[4 + i] = __ldg(wpB + i); }
-    }
-  }
-  tmem_ld_wait(acc);
-  TSTAMP(t1);
-#ifdef STNERF_TIMING
-  long long t2 = t1, t3 = t1;
-#endif
-#pragma unroll
-  for (int pass = 0; pass < 2; ++pass) {
-    float v[16];
-    uint32_t hp[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {                      // HI: bias, ReLU, fp16 -- two 16-byte chunks of 8 columns
-      const int c = pass * 16 + e * 2;
-      const float4 bb = bv[c >> 2];
-      const float b0 = (c & 2) ? bb.z : bb.x, b1 = (c & 2) ? bb.w : bb.y;
-      v[2 * e] = fmaxf(__uint_as_float(acc[c]) + b0, 0.f);
-      v[2 * e + 1] = fmaxf(__uint_as_float(acc[c + 1]) + b1, 0.f);
-      hp[e] = pack_f16x2(v[2 * e], v[2 * e + 1]);
-    }
-    const uint32_t off0 = sw128_offset(row, pass * 32 + hh * 16), off1 = sw128_offset(row, pass * 32 + hh * 16 + 8);
-    const uint32_t tcol = dcol + (uint32_t)(pass ? colB : colA);
-    if (ATMEM) {
-      tmem_st8(tcol, hp);
-      tmem_st_wait();
-      tc_fence_before();
-    } else {
-      *reinterpret_cast<uint4*>(blk + off0) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-      *reinterpret_cast<uint4*>(blk + off1) = make_uint4(hp[4], hp[5], hp[6], hp[7]);
-      fence_proxy_async();
-    }
-    __syncwarp();
-    if (lane == 0) { if (PAIR) mbar_arrive_cluster(ready_bar + 8u * pass); else mbar_arrive(ready_bar + 8u * pass); }
-    if (exact) {                                       // LO: what the fp16 rounding of HI left over
-      uint32_t lp[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float2 hf = unpack_f16x2(hp[e]);
-        lp[e] = pack_f16x2(v[2 * e] - hf.x, v[2 * e + 1] - hf.y);
-      }
-      if (ATMEM) {
-        tmem_st8(tcol + 8u, lp);
-      } else {
-        *reinterpret_cast<uint4*>(blk + lo_stride + off0) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
-        *reinterpret_cast<uint4*>(blk + lo_stride + off1) = make_uint4(lp[4], lp[5], lp[6], lp[7]);
-      }
-    }
-    if (SIGMA) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int c = pass * 16 + e * 2;
-        const float4 ww = wv[c >> 2];
-        dot = fmaf(v[2 * e], (c & 2) ? ww.z : ww.x, dot);
-        dot = fmaf(v[2 * e + 1], (c & 2) ? ww.w : ww.y, dot);
-      }
-    }
-#ifdef STNERF_TIMING
-    if (pass == 1) t2 = clock64();
-#endif
-    if (ATMEM) {
-      if (exact) tmem_st_wait();
-      tc_fence_before();
-    } else if (exact) {
-      fence_proxy_async();
-    }
-    __syncwarp();
-#ifdef STNERF_TIMING
-    if (pass == 1) t3 = clock64();
-#endif
-    if (lane == 0) {
-      if (PAIR) mbar_arrive_cluster(ready_bar + 8u * (AREADY_LO + pass)); else mbar_arrive(ready_bar + 8u * (AREADY_LO + pass));
-    }
-  }
-#ifdef STNERF_TIMING
-  const long long t4 = clock64();
-  tm.ld += t1 - t0; tm.math += t2 - t1; tm.fence += t3 - t2; tm.arrive += t4 - t3; tm.n += 1;
-#endif
-  return dot;
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // coarse-pass fusion: what the two spare warps of the SpaceNet kernel run (see FuseCoarse in mlp_tc.cuh)
 // ---------------------------------------------------------------------------------------------------------
@@ -864,23 +515,129 @@ __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// the kernel
+// the kernel: one layer of a math warpgroup
 // ---------------------------------------------------------------------------------------------------------
-// PAIR: the two CTAs of a cluster share ONE M = 256 accumulator (`cta_group::2`).  Each CTA still owns a 128-point tile -- its
-// activations, its TMEM rows, its epilogue -- but streams only HALF of every weight stage (the B rows of its half of the
-// output columns); the leader (cluster rank 0) issues the MMAs for both, so per SM the B operand reads and the L2 -> shared
-// weight traffic are halved.  Barriers the leader's MMA warp waits on collect arrivals from both CTAs (remote arrives);
-// `tcgen05.commit` multicasts to the same barrier in both CTAs.
-// WSHARE: the two CTAs of a cluster keep their own tiles, accumulators and MMAs (cta_group::1) but share the WEIGHT STREAM: CTA r
-// pulls rows [r*N/2, (r+1)*N/2) of every stage from L2 and multicasts them into both shared memories, so the L2 -> SM traffic per
-// SM halves.  A ring slot is refilled once BOTH CTAs' MMAs on it have retired (multicast commits on w_empty, count 2).
-template <int NET, bool PAIR = false, bool WSHARE = false, bool LOFIRST = false>
-__global__ void __launch_bounds__(Sched<NET>::N_THREADS, Sched<NET>::CTAS_PER_SM) mlp_tc_kernel(const __grid_constant__ TcParams P) {
+// MMAs of layer l for this warpgroup's 64 rows (A rows at byte offset a_row of every activation / encoding block), consuming the
+// weight stages in the order the producer streams them.  A stage is handed back (one arrival per math warp on w_empty) once the
+// MMAs that read it have retired: wgmma.wait_group 1 after the next stage's MMAs are issued keeps one stage of MMAs in flight.
+template <int NET, int N, bool LOFIRST>
+__device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uint32_t sbase, uint32_t a_row, uint32_t bars,
+                                          uint32_t& cnt, int lane) {
   using S = Sched<NET>;
-  static_assert(!PAIR || NET == NET_SPACE, "the CTA-pair protocol is built for the SpaceNet schedule");
-  static_assert(!(PAIR && WSHARE) && (!WSHARE || NET == NET_SPACE), "weight sharing is a SpaceNet-only alternative to the pair protocol");
-  const uint32_t rank = (PAIR || WSHARE) ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
+  constexpr uint32_t NST = S::n_stage;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  acc_fence<N / 2>(acc);
+  wgmma_fence();
+  const int nact = S::act_chunks(l), nch = nact + S::enc_chunks(l);
+  int pend = -1;
+  auto release = [&](int s) {
+    __syncwarp();
+    mbar_arrive_if(bars + 8u * (uint32_t)(BAR_WEMPTY + s), lane == 0);
+  };
+  // the next weight stage of the stream times the 32-k slice at a0 (and, two == true, at a1 as well)
+  auto stage = [&](uint32_t a0, uint32_t a1, auto two) {
+    const uint32_t s = cnt % NST, n = cnt / NST;
+    mbar_wait(bars + 8u * (BAR_WFULL + s), n & 1);
+    const uint32_t w = sbase + S::ring_base + s * S::stage_bytes;
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a0 + ks * 32), desc_sw64(w + ks * 32));
+    if (decltype(two)::value) {
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a1 + ks * 32), desc_sw64(w + ks * 32));
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (pend >= 0) release(pend);
+    pend = (int)s;
+    ++cnt;
+  };
+  // hi / lo halves of A chunk ch (64 k): activation chunks 0..nact-1, then the encoding chunks
+  auto a_block = [&](int ch, uint32_t& hi, uint32_t& lo) {
+    if (ch < nact) {
+      hi = sbase + S::act_base + ch * ABLOCK + a_row;
+      lo = hi + S::LO_STRIDE;
+    } else {
+      hi = sbase + S::enc_base + (ch - nact) * ABLOCK + a_row;
+      lo = hi + S::ENC_LO_STRIDE;
+    }
+  };
+  // position c of the layer's K order -> chunk id
+  auto chunk_at = [&](int c) { return (S::enc_first(l) && nact > 0 && nch > nact) ? (c == 0 ? nact : c - 1) : c; };
+  if (!LOFIRST || !sp) {
+    // interleaved order (and single-pass layers): per 32-k sub-chunk Ahi*Wlo off the lo stage, then Ahi*Whi and Alo*Whi off the hi stage
+    for (int c = 0; c < nch; ++c) {
+      uint32_t hi, lo;
+      a_block(chunk_at(c), hi, lo);
+      for (uint32_t sub = 0; sub < 2; ++sub) {
+        if (sp) {
+          stage(hi + 64u * sub, 0u, std::false_type());
+          stage(hi + 64u * sub, lo + 64u * sub, std::true_type());
+        } else {
+          stage(hi + 64u * sub, 0u, std::false_type());
+        }
+      }
+    }
+  } else {
+    // corrections first: D = Ahi*Wlo + Alo*Whi over the whole K range, then D += Ahi*Whi off the main section
+    for (int c = 0; c < nch; ++c) {
+      uint32_t hi, lo;
+      a_block(chunk_at(c), hi, lo);
+      for (uint32_t sub = 0; sub < 2; ++sub) {
+        stage(hi + 64u * sub, 0u, std::false_type());          // lo weight stage
+        stage(lo + 64u * sub, 0u, std::false_type());          // hi weight stage
+      }
+    }
+    for (int c = 0; c < nch; ++c) {
+      uint32_t hi, lo;
+      a_block(chunk_at(c), hi, lo);
+      for (uint32_t sub = 0; sub < 2; ++sub) stage(hi + 64u * sub, 0u, std::false_type());
+    }
+  }
+  wgmma_wait<0>();
+  acc_fence<N / 2>(acc);
+  release(pend);
+}
+
+// Hidden-layer epilogue from the accumulator fragment: bias, ReLU, fp16 hi (+ lo) split into the activation blocks (rows r0 and
+// r0 + 8, columns 8 j + cq, +1 for j < N / 8); SIGMA: the density head's partial dot products of the two rows.
+template <int NET, int N, bool SIGMA>
+__device__ __forceinline__ void epi_hidden(const float (&acc)[128], const float* __restrict__ bias, const float* __restrict__ wsig,
+                                           uint8_t* smem, int r0, int cq, bool lo_too, float& sig0, float& sig1) {
+  using S = Sched<NET>;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = 8 * j + cq;
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+    const float v00 = fmaxf(acc[4 * j] + b.x, 0.f), v01 = fmaxf(acc[4 * j + 1] + b.y, 0.f);
+    const float v10 = fmaxf(acc[4 * j + 2] + b.x, 0.f), v11 = fmaxf(acc[4 * j + 3] + b.y, 0.f);
+    if (SIGMA) {
+      const float2 w = __ldg(reinterpret_cast<const float2*>(wsig + col));
+      sig0 = fmaf(v00, w.x, sig0); sig0 = fmaf(v01, w.y, sig0);
+      sig1 = fmaf(v10, w.x, sig1); sig1 = fmaf(v11, w.y, sig1);
+    }
+    uint8_t* blk = smem + S::act_base + (col >> 6) * ABLOCK;
+    const uint32_t o0 = sw128_offset(r0, col & 63), o1 = sw128_offset(r0 + 8, col & 63);
+    const uint32_t h0 = pack_f16x2(v00, v01), h1 = pack_f16x2(v10, v11);
+    *reinterpret_cast<uint32_t*>(blk + o0) = h0;
+    *reinterpret_cast<uint32_t*>(blk + o1) = h1;
+    if (lo_too) {
+      const float2 f0 = unpack_f16x2(h0), f1 = unpack_f16x2(h1);
+      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o0) = pack_f16x2(v00 - f0.x, v01 - f0.y);
+      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o1) = pack_f16x2(v10 - f1.x, v11 - f1.y);
+    }
+  }
+}
+
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+template <int NET, bool LOFIRST>
+__global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_constant__ TcParams P) {
+  using S = Sched<NET>;
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
   if ((sbase & 1023u) != 0) {                    // swizzled operands need a 1024-byte aligned base
@@ -889,69 +646,50 @@ __global__ void __launch_bounds__(Sched<NET>::N_THREADS, Sched<NET>::CTAS_PER_SM
   }
   const uint32_t bars = sbase + S::misc_base;
   auto BAR = [bars](int i) { return bars + 8u * (uint32_t)i; };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + S::misc_base + MISC_TMEM);
-  float* s_part = reinterpret_cast<float*>(smem + S::misc_base + MISC_PART);     // [128][4]
+  Pt* s_rows = reinterpret_cast<Pt*>(smem + S::misc_base + MISC_ROWS);          // the current tile's points (per math warpgroup rows)
+  float* s_part = reinterpret_cast<float*>(smem + S::misc_base + MISC_PART);    // [128][4]
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  // warp and warpgroup indices broadcast from lane 0: the compiler then knows every role branch below is warp-uniform, and the
+  // warpgroup MMAs inside them are not serialized as if they sat on a divergent path
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int wgi = __shfl_sync(0xffffffffu, tid >> 7, 0);
   const bool exact = P.exact != 0;
   // 3-term split for layer l?  (mixed mode: everything the density depends on is split, the colour-only layer is not)
   const bool single_last = P.single_last != 0;
   auto split = [&](int l) { return exact && !(single_last && l == S::N_LAYERS - 1); };
-  // hidden activations in tensor memory (see SPACE_A_TMEM); the encoding chunks (layer 0, skip layer) stay in shared memory
-  constexpr bool ATMEM = (NET == NET_SPACE) && !PAIR && (SPACE_A_TMEM != 0);
-  constexpr bool lo_first = LOFIRST;      // order of the split MMAs: a compile-time variant, the interleaved default pays nothing for it
   const long long n_points = src_num_points(P.src);
   const long long n_tiles = (n_points + TILE_M - 1) / TILE_M;
-
-  constexpr uint32_t N_ARRIVE = PAIR ? 2 * N_EPI_WARPS : N_EPI_WARPS;      // epilogue warps of both CTAs report to the leader
-  // weight ring: a CTA of a pair holds half of every stage, so the same 64 KB give twice the slots -- the extra depth pays
-  // for the relay hop (peer's copy lands -> remote arrive -> leader) on top of the L2 latency
-  constexpr uint32_t NST = PAIR ? 2 * NSTAGE : S::n_stage;
-  constexpr uint32_t STAGE_STRIDE = PAIR ? S::stage_bytes / 2 : S::stage_bytes;
-  static_assert(NST <= MAX_STAGE, "barrier slots");
+  constexpr uint32_t NST = S::n_stage;
   if (tid == 0) {
-    for (int i = 0; i < MAX_STAGE; ++i) { mbar_init(BAR(BAR_WFULL + i), 1); mbar_init(BAR(BAR_WEMPTY + i), WSHARE ? 2 : 1); mbar_init(BAR(BAR_WPEER + i), 1); }
-    for (int i = 0; i < N_AREADY; ++i) mbar_init(BAR(BAR_AREADY + i), N_ARRIVE);
-    for (int i = 0; i < 2; ++i) { mbar_init(BAR(BAR_DFULL + i), 1); mbar_init(BAR(BAR_DEMPTY + i), N_ARRIVE); }
-    mbar_init(BAR(BAR_RAWFULL), 4);          // the four epilogue warps that own the tile's final rows
-    mbar_init(BAR(BAR_RAWEMPTY), 2);         // the two compositing warps
+    for (int i = 0; i < MAX_STAGE; ++i) { mbar_init(BAR(BAR_WFULL + i), 1); mbar_init(BAR(BAR_WEMPTY + i), N_MATH_WARPS); }
+    for (int j = 0; j < 2; ++j) {
+      mbar_init(BAR(BAR_RAWFULL + j), 4);          // the four warps of math warpgroup j (its 64 rows = one ray)
+      mbar_init(BAR(BAR_RAWEMPTY + j), 1);         // compositing warp j
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) { if (PAIR) tmem_alloc_pair(smem_u32(tmem_slot), S::tmem_cols); else tmem_alloc(smem_u32(tmem_slot), S::tmem_cols); }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR || WSHARE) cluster_sync_all();        // the peer's barriers exist before anyone arrives on them remotely
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // barrier `i` as the LEADER sees it (what the epilogue warps of either CTA arrive on)
-  auto LBAR = [&](int i) { return PAIR ? map_to_cta(BAR(i), 0) : BAR(i); };
-  // tiles: CTA b takes tiles b, b + grid, ...; the CTAs of a pair run the same number of rounds (the odd one out gets a tile
-  // past the end, whose points are all invalid)
-  auto in_range = [&](long long tile) { return (PAIR || WSHARE) ? ((tile & ~1LL) < n_tiles) : (tile < n_tiles); };
 
-  if (warp == 0 && !PAIR && PRODUCER_ELECT) {
+  if (warp == 0) {
     // =============================== weight producer: the whole warp runs the loop, one elected lane issues ===============================
     uint32_t cnt = 0;
-    for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x) {
+    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       const uint8_t* src = P.wstream;
       for (int l = 0; l < S::N_LAYERS; ++l) {
         const int nsub = 2 * (S::act_chunks(l) + S::enc_chunks(l));
         const uint32_t bytes = (uint32_t)S::n_out(l) * 64;
         const bool sp = split(l);
-        // WSHARE: the whole stage lands in both CTAs (half from this CTA's copy, half from the peer's); this CTA issues its half to both
         auto LOAD = [&](const uint8_t* stage) {
           const uint32_t s = cnt % NST, n = cnt / NST;
           mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
-          const uint32_t dst = sbase + S::ring_base + s * STAGE_STRIDE;
-          if (WSHARE) load_stage_elect<true>(dst + rank * (bytes / 2), stage + rank * (bytes / 2), bytes / 2, bytes, BAR(BAR_WFULL + s));
-          else load_stage_elect<false>(dst, stage, bytes, bytes, BAR(BAR_WFULL + s));
+          load_stage_elect(sbase + S::ring_base + s * S::stage_bytes, stage, bytes, BAR(BAR_WFULL + s));
           ++cnt;
         };
-        // a layer of the stream = correction section [(hi, lo) per 32-k sub-chunk] + main section [hi per sub-chunk] (see the MMA warp)
+        // a layer of the stream = correction section [(hi, lo) per 32-k sub-chunk] + main section [hi per sub-chunk]
         const uint8_t* corr = src;
         const uint8_t* mainp = src + (size_t)nsub * 2 * bytes;
-        // The stream stores (hi, lo) per sub-chunk; the lo stage is CONSUMED first (Ahi*Wlo needs only the HI half of A, which the
-        // epilogue hands over first), so it is loaded first.
+        // the lo stage is consumed first (Ahi*Wlo), so it is loaded first
         if (!LOFIRST) {       // interleaved order: the (lo, hi) stages of the correction section serve all three products;
           for (int sc = 0; sc < nsub; ++sc) {                      // single-pass layers never touch the lo stages
             if (sp) LOAD(corr + (size_t)(2 * sc + 1) * bytes);
@@ -965,570 +703,121 @@ __global__ void __launch_bounds__(Sched<NET>::N_THREADS, Sched<NET>::CTAS_PER_SM
         src = mainp + (size_t)nsub * bytes;
       }
     }
-  } else if (warp == 0) {
-    // =============================== weight producer (single lane: CTA-pair build, PRODUCER_ELECT=0) ===============================
-    if (lane == 0) {
-      uint32_t cnt = 0;
-      for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x) {
-        const uint8_t* src = P.wstream;
-        for (int l = 0; l < S::N_LAYERS; ++l) {
-          const int nsub = 2 * (S::act_chunks(l) + S::enc_chunks(l));
-          const uint32_t bytes = (uint32_t)S::n_out(l) * 64;
-          const uint32_t mine = PAIR ? bytes / 2 : bytes;     // pair: the rows of this CTA's half of the output columns
-          // a layer of the stream = correction section [(hi, lo) per 32-k sub-chunk] + main section [hi per sub-chunk] (see the MMA warp)
-          if (!LOFIRST) {     // interleaved order: the (hi, lo) stages of the correction section serve all three products
-            for (int sc = 0; sc < nsub; ++sc, src += 2 * (size_t)bytes)
-              for (int term = 0; term < 2; ++term) {             // the lo stage (stored second) is consumed, hence loaded, first
-                if (term == 0 && !split(l)) continue;            // single-pass layers never touch the lo stages
-                const uint8_t* stage = src + (term == 0 ? bytes : 0u);
-                const uint32_t s = cnt % NST, n = cnt / NST;
-                mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
-                if (WSHARE) {      // the whole stage lands here (half from this CTA's copy, half from the peer's); this CTA issues its half to both
-                  mbar_expect_tx(BAR(BAR_WFULL + s), bytes);
-                  bulk_g2s_mc(sbase + S::ring_base + s * STAGE_STRIDE + rank * (bytes / 2), stage + rank * (bytes / 2), bytes / 2,
-                              BAR(BAR_WFULL + s), (uint16_t)3);
-                  ++cnt;
-                  continue;
-                }
-                mbar_expect_tx(BAR(BAR_WFULL + s), mine);
-                bulk_g2s(sbase + S::ring_base + s * STAGE_STRIDE, stage + (PAIR ? rank * mine : 0u), mine, BAR(BAR_WFULL + s));
-                ++cnt;
-              }
-            src += (size_t)nsub * bytes;      // the main section is not used
-          } else {
-            auto LOAD = [&](const uint8_t* stage) {
-              const uint32_t s = cnt % NST, n = cnt / NST;
-              mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
-              if (WSHARE) {      // the whole stage lands here (half from this CTA's copy, half from the peer's); this CTA issues its half to both
-                mbar_expect_tx(BAR(BAR_WFULL + s), bytes);
-                bulk_g2s_mc(sbase + S::ring_base + s * STAGE_STRIDE + rank * (bytes / 2), stage + rank * (bytes / 2), bytes / 2,
-                            BAR(BAR_WFULL + s), (uint16_t)3);
-              } else {
-                mbar_expect_tx(BAR(BAR_WFULL + s), mine);
-                bulk_g2s(sbase + S::ring_base + s * STAGE_STRIDE, stage + (PAIR ? rank * mine : 0u), mine, BAR(BAR_WFULL + s));
-              }
-              ++cnt;
-            };
-            const uint8_t* corr = src;
-            const uint8_t* mainp = src + (size_t)nsub * 2 * bytes;
-            if (split(l))
-              for (int sc = 0; sc < nsub; ++sc) { LOAD(corr + (size_t)(2 * sc + 1) * bytes); LOAD(corr + (size_t)(2 * sc) * bytes); }
-            for (int sc = 0; sc < nsub; ++sc) LOAD(mainp + (size_t)sc * bytes);
-            src = mainp + (size_t)nsub * bytes;
-          }
-        }
-      }
-    }
-  } else if (warp == 1 && PAIR && !leader) {
-    // =============================== peer of a pair: relay "my half of stage s has landed" to the leader ===============
-    if (lane == 0) {
-      uint32_t cnt = 0;
-      for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x)
-        for (int l = 0; l < S::N_LAYERS; ++l) {
-          const int nsub = 2 * (S::act_chunks(l) + S::enc_chunks(l));
-          const int nstages = split(l) ? (lo_first ? 3 : 2) * nsub : nsub;
-          for (int k = 0; k < nstages; ++k) {
-            const uint32_t s = cnt % NST, n = cnt / NST;
-            mbar_wait(BAR(BAR_WFULL + s), n & 1);
-            mbar_arrive_cluster(map_to_cta(BAR(BAR_WPEER + s), 0));
-            ++cnt;
-          }
-        }
-    }
-  } else if (warp == 1 && !PAIR) {
-    // =============================== MMA issuer: the whole warp runs the loop, one elected lane issues ===============================
-    uint32_t cnt = 0;            // weight stages consumed
-    uint32_t g = 0;              // global layer counter (selects the TMEM buffer)
-    uint32_t a_par = 0;          // phase parity of a_ready[0..16], one bit each
-    for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x) {
-      for (int l = 0; l < S::N_LAYERS; ++l, ++g) {
-        const uint32_t b = g & 1;
-        mbar_wait(BAR(BAR_DEMPTY + b), ((g >> 1) & 1) ^ 1);          // accumulator buffer drained (layer g-2)
-        tc_fence_after();
-        const uint32_t d = tmem_base + b * S::d_stride;
-        const uint32_t idesc = idesc_n((uint32_t)S::n_out(l));
-        const int nact = S::act_chunks(l), nch = nact + S::enc_chunks(l);
-        const bool sp = split(l);
-        uint32_t acc = 0;        // the first MMA of the layer overwrites the accumulator
-        // ATMEM: this layer's accumulator buffer is the one the PREVIOUS layer's MMAs read their A operand from.  A layer that opens
-        // with an activation chunk waits for the previous layer's epilogue anyway (hence for d_full); one that opens with the
-        // encoding (layer 0 after the last layer of the previous tile, the skip layer) waits for the previous MMAs to retire here.
-        if (ATMEM && g > 0 && (l == 0 || S::enc_first(l))) {
-          mbar_wait(BAR(BAR_DFULL + (b ^ 1u)), ((g - 1) >> 1) & 1);
-          tc_fence_after();
-        }
-        // descriptor words of the hi / lo halves of A chunk c (64 k) and the a_ready barriers of its two 32-k sub-chunks: bar[sub] for
-        // the HI half, bar[sub] + AREADY_LO for the LO half (-1: none; the encoding has ONE arrival phase per tile, hi and lo
-        // together, waited for at its first use: layer 0, chunk 0, sub-chunk 0)
-        auto a_block = [&](int c, uint32_t& a_hi, uint32_t& a_lo, int& bar0, int& bar1, bool& has_lo_bar) {
-          uint32_t addr, lo_stride;
-          if (c < nact) {
-            bar0 = 2 * c; bar1 = 2 * c + 1; has_lo_bar = true;
-            if (ATMEM) {       // the previous layer's accumulator buffer, converted in place: tensor-memory column of k = 64 c
-              a_hi = tmem_base + (b ^ 1u) * S::d_stride + (uint32_t)c * 64u;
-              a_lo = a_hi + 8u;
-              return;
-            }
-            addr = sbase + S::act_base + c * ABLOCK; lo_stride = S::LO_STRIDE;
-          } else {
-            const int e = c - nact;
-            addr = sbase + S::enc_base + e * ABLOCK; lo_stride = S::ENC_LO_STRIDE;
-            bar0 = (l == 0 && e == 0) ? AREADY_ENC : -1; bar1 = -1; has_lo_bar = false;
-          }
-          a_hi = desc_lo(addr);
-          a_lo = desc_lo(addr + lo_stride);
-        };
-        // position c of the layer's K order -> chunk id (activation chunks 0..nact-1, then the encoding chunks)
-        auto chunk_at = [&](int c) { return (S::enc_first(l) && nact > 0 && nch > nact) ? (c == 0 ? nact : c - 1) : c; };
-        auto a_wait = [&](int bar_i) {           // the epilogue (or the encoder) has written this sub-chunk of the A operand
-          if (bar_i < 0) return;
-          mbar_wait(BAR(BAR_AREADY + bar_i), (a_par >> bar_i) & 1u);
-          a_par ^= 1u << bar_i;
-          tc_fence_after();
-        };
-        // the next weight stage of the stream times the 32-k slice(s) of A at descriptor word(s) a0 (and a1)
-        // (ts: the slices are tensor-memory addresses -- activation chunks under ATMEM)
-        auto stage2 = [&](uint32_t a0, bool ts) {
-          const uint32_t s = cnt % NST, n = cnt / NST;
-          mbar_wait(BAR(BAR_WFULL + s), n & 1);
-          if (ATMEM && ts) issue_stage_ts<1, WSHARE>(d, a0, a0, desc_lo(sbase + S::ring_base + s * STAGE_STRIDE), idesc, acc, BAR(BAR_WEMPTY + s));
-          else issue_stage<1, WSHARE>(d, a0, a0, desc_lo(sbase + S::ring_base + s * STAGE_STRIDE), idesc, acc, BAR(BAR_WEMPTY + s));
-          acc = 1; ++cnt;
-        };
-        auto stage4 = [&](uint32_t a0, uint32_t a1, bool ts) {
-          const uint32_t s = cnt % NST, n = cnt / NST;
-          mbar_wait(BAR(BAR_WFULL + s), n & 1);
-          if (ATMEM && ts) issue_stage_ts<2, WSHARE>(d, a0, a1, desc_lo(sbase + S::ring_base + s * STAGE_STRIDE), idesc, acc, BAR(BAR_WEMPTY + s));
-          else issue_stage<2, WSHARE>(d, a0, a1, desc_lo(sbase + S::ring_base + s * STAGE_STRIDE), idesc, acc, BAR(BAR_WEMPTY + s));
-          acc = 1; ++cnt;
-        };
-        if (!LOFIRST || !sp) {
-          // interleaved order (and single-pass layers): per 32-k sub-chunk Ahi*Wlo off the lo stage -- needs only the HI half of A, which
-          // the epilogue delivers first -- then Ahi*Whi and Alo*Whi off the hi stage
-          for (int c = 0; c < nch; ++c) {
-            uint32_t a_hi, a_lo;
-            int bar[2];
-            bool lo_bar;
-            a_block(chunk_at(c), a_hi, a_lo, bar[0], bar[1], lo_bar);
-            const bool ts = ATMEM && lo_bar;                          // activation chunk in tensor memory
-            const uint32_t sstep = ts ? 32u : 4u;                     // next 32-k sub-chunk: 32 columns / 64 bytes along K (+4 in the address field)
-#pragma unroll
-            for (uint32_t sub = 0; sub < 2; ++sub) {
-              a_wait(bar[sub]);
-              if (sp) {
-                stage2(a_hi + sstep * sub, ts);                        // lo weight stage
-                if (lo_bar) a_wait(AREADY_LO + bar[sub]);
-                stage4(a_hi + sstep * sub, a_lo + sstep * sub, ts);    // hi weight stage
-              } else {
-                if (lo_bar) a_wait(AREADY_LO + bar[sub]);              // (keeps the barrier's phase in step; nothing is read)
-                stage2(a_hi + sstep * sub, ts);
-              }
-            }
-          }
-        } else {
-          // corrections first (see the file header): D = Ahi*Wlo + Alo*Whi over the whole K range, then D += Ahi*Whi off the main section
-          for (int c = 0; c < nch; ++c) {
-            uint32_t a_hi, a_lo;
-            int bar[2];
-            bool lo_bar;
-            a_block(chunk_at(c), a_hi, a_lo, bar[0], bar[1], lo_bar);
-            const bool ts = ATMEM && lo_bar;
-            const uint32_t sstep = ts ? 32u : 4u;
-#pragma unroll
-            for (uint32_t sub = 0; sub < 2; ++sub) {
-              a_wait(bar[sub]);
-              stage2(a_hi + sstep * sub, ts);                          // lo weight stage
-              if (lo_bar) a_wait(AREADY_LO + bar[sub]);
-              stage2(a_lo + sstep * sub, ts);                          // hi weight stage
-            }
-          }
-          for (int c = 0; c < nch; ++c) {
-            uint32_t a_hi, a_lo;
-            int bar[2];
-            bool lo_bar;
-            a_block(chunk_at(c), a_hi, a_lo, bar[0], bar[1], lo_bar);
-            const bool ts = ATMEM && lo_bar;
-            const uint32_t sstep = ts ? 32u : 4u;
-#pragma unroll
-            for (uint32_t sub = 0; sub < 2; ++sub) stage2(a_hi + sstep * sub, ts);
-          }
-        }
-        commit_elect(BAR(BAR_DFULL + b));                              // accumulator of layer g complete
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer (CTA-pair build: single lane, cta_group::2) ===============================
-    if (lane == 0) {
-      uint32_t cnt = 0;            // weight stages consumed
-      uint32_t g = 0;              // global layer counter (selects the TMEM buffer)
-      uint32_t a_uses[N_AREADY] = {};
-      auto WAIT = [&](uint32_t bar, uint32_t parity) { if (PAIR) mbar_wait_cluster(bar, parity); else mbar_wait(bar, parity); };
-      for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x) {
-        for (int l = 0; l < S::N_LAYERS; ++l, ++g) {
-          const uint32_t b = g & 1;
-          WAIT(BAR(BAR_DEMPTY + b), ((g >> 1) & 1) ^ 1);           // accumulator buffer drained (layer g-2)
-          tc_fence_after();
-          const uint32_t d = tmem_base + b * S::d_stride;
-          const uint32_t idesc = PAIR ? idesc_pair_n((uint32_t)S::n_out(l)) : idesc_n((uint32_t)S::n_out(l));
-          const int nact = S::act_chunks(l), nch = nact + S::enc_chunks(l);
-          if (!LOFIRST) {
-            // interleaved order: per 32-k sub-chunk, Ahi*Whi and Alo*Whi off the hi stage, Ahi*Wlo off the lo stage
-            for (int cpos = 0; cpos < nch; ++cpos) {
-              const int c = (S::enc_first(l) && nact > 0 && nch > nact) ? (cpos == 0 ? nact : cpos - 1) : cpos;
-              uint32_t a_hi, a_lo;
-              if (c < nact) {
-                a_hi = sbase + S::act_base + c * ABLOCK;
-                a_lo = a_hi + S::LO_STRIDE;
-                for (int i = 0; i < 4; ++i) {                        // both 32-k sub-chunks of the chunk, hi and lo halves
-                  const int bi = 2 * c + (i & 1) + (i >> 1) * AREADY_LO;
-                  WAIT(BAR(BAR_AREADY + bi), a_uses[bi] & 1);
-                  ++a_uses[bi];
-                }
-              } else {
-                const int e = c - nact;
-                a_hi = sbase + S::enc_base + e * ABLOCK;
-                a_lo = a_hi + S::ENC_LO_STRIDE;
-                if (l == 0 && e == 0) {                              // one arrival phase per tile covers the whole encoding
-                  WAIT(BAR(BAR_AREADY + AREADY_ENC), a_uses[AREADY_ENC] & 1);
-                  ++a_uses[AREADY_ENC];
-                }
-              }
-              tc_fence_after();
-              for (int sub = 0; sub < 2; ++sub) {
-                const uint32_t a_off = (uint32_t)sub * 64;           // two 32-byte k-steps per 32-wide sub-chunk
-                for (int term = 1; term >= 0; --term) {              // the lo stage comes first in the ring (see the producer)
-                  if (term == 1 && !split(l)) continue;
-                  const bool first_mma = (cpos == 0 && sub == 0 && term == (split(l) ? 1 : 0));
-                  const uint32_t s = cnt % NST, n = cnt / NST;
-                  mbar_wait(BAR(BAR_WFULL + s), n & 1);
-                  if (PAIR) mbar_wait_cluster(BAR(BAR_WPEER + s), n & 1);      // ... and the peer's half
-                  tc_fence_after();
-                  const uint32_t wsm = sbase + S::ring_base + s * STAGE_STRIDE;
-                  // hi stage: D += Ahi*Whi (+ Alo*Whi);  lo stage: D += Ahi*Wlo
-                  auto MMA = [&](uint32_t a_addr, int ks, uint32_t acc) {
-                    if (PAIR) umma_f16_pair(d, make_desc_sw128(a_addr + ks * 32), make_desc_sw64(wsm + ks * 32), idesc, acc);
-                    else umma_f16(d, make_desc_sw128(a_addr + ks * 32), make_desc_sw64(wsm + ks * 32), idesc, acc);
-                  };
-#pragma unroll
-                  for (int ks = 0; ks < 2; ++ks) MMA(a_hi + a_off, ks, (first_mma && ks == 0) ? 0u : 1u);
-                  if (term == 0 && split(l)) {
-#pragma unroll
-                    for (int ks = 0; ks < 2; ++ks) MMA(a_lo + a_off, ks, 1u);
-                  }
-                  if (PAIR) umma_commit_pair(BAR(BAR_WEMPTY + s));    // ring slot (of both CTAs) reusable once these MMAs retire
-                  else if (WSHARE) umma_commit_mc(BAR(BAR_WEMPTY + s), (uint16_t)3);   // ... this CTA's MMAs: one of the two arrivals, in both CTAs
-                  else umma_commit(BAR(BAR_WEMPTY + s));
-                  ++cnt;
-                }
-              }
-            }
-          } else {
-            // Order of the MMAs of a layer.  The tensor core TRUNCATES when it adds into the fp32 accumulator (measured:
-            // stnerf_selftest_umma_accum), an error relative to the accumulator's magnitude at that moment.  So the two correction
-            // products go FIRST, over the whole K range, while the accumulator only holds terms 2^-11 of its final size; the main
-            // product Ahi*Whi follows.  A layer then truncates at full magnitude K/16 times instead of 3K/16 times; the price is a
-            // second copy of the hi weight stages in the stream (main section).
-            bool first = true;
-            auto chunk = [&](int c, bool wait, uint32_t& a_hi, uint32_t& a_lo) {
-              if (c < nact) {
-                a_hi = sbase + S::act_base + c * ABLOCK;
-                a_lo = a_hi + S::LO_STRIDE;
-                if (wait) {
-                  for (int i = 0; i < 4; ++i) {                      // both 32-k sub-chunks of the chunk, hi and lo halves
-                    const int bi = 2 * c + (i & 1) + (i >> 1) * AREADY_LO;
-                    WAIT(BAR(BAR_AREADY + bi), a_uses[bi] & 1);
-                    ++a_uses[bi];
-                  }
-                }
-              } else {
-                const int e = c - nact;
-                a_hi = sbase + S::enc_base + e * ABLOCK;
-                a_lo = a_hi + S::ENC_LO_STRIDE;
-                if (wait && l == 0 && e == 0) {                      // one arrival phase per tile covers the whole encoding
-                  WAIT(BAR(BAR_AREADY + AREADY_ENC), a_uses[AREADY_ENC] & 1);
-                  ++a_uses[AREADY_ENC];
-                }
-              }
-              if (wait) tc_fence_after();
-            };
-            // the next weight stage of the stream times the 32-k slice at a_addr
-            auto STAGE = [&](uint32_t a_addr) {
-              const uint32_t s = cnt % NST, n = cnt / NST;
-              mbar_wait(BAR(BAR_WFULL + s), n & 1);
-              if (PAIR) mbar_wait_cluster(BAR(BAR_WPEER + s), n & 1);        // ... and the peer's half
-              tc_fence_after();
-              const uint32_t wsm = sbase + S::ring_base + s * STAGE_STRIDE;
-#pragma unroll
-              for (int ks = 0; ks < 2; ++ks) {
-                const uint32_t acc = first ? 0u : 1u;
-                first = false;
-                if (PAIR) umma_f16_pair(d, make_desc_sw128(a_addr + ks * 32), make_desc_sw64(wsm + ks * 32), idesc, acc);
-                else umma_f16(d, make_desc_sw128(a_addr + ks * 32), make_desc_sw64(wsm + ks * 32), idesc, acc);
-              }
-              if (PAIR) umma_commit_pair(BAR(BAR_WEMPTY + s));        // ring slot (of both CTAs) reusable once these MMAs retire
-              else if (WSHARE) umma_commit_mc(BAR(BAR_WEMPTY + s), (uint16_t)3);   // this CTA's MMAs: one of the two arrivals, in both CTAs
-              else umma_commit(BAR(BAR_WEMPTY + s));
-              ++cnt;
-            };
-            const bool sp = split(l);
-            if (sp) {
-              for (int c = 0; c < nch; ++c) {
-                uint32_t a_hi, a_lo;
-                chunk((S::enc_first(l) && nact > 0 && nch > nact) ? (c == 0 ? nact : c - 1) : c, true, a_hi, a_lo);
-                for (int sub = 0; sub < 2; ++sub) {                  // correction pass: D = Ahi*Wlo + Alo*Whi
-                  STAGE(a_hi + (uint32_t)sub * 64);                  // lo weight stage
-                  STAGE(a_lo + (uint32_t)sub * 64);                  // hi weight stage
-                }
-              }
-            }
-            for (int c = 0; c < nch; ++c) {                          // main pass: D += Ahi*Whi
-              uint32_t a_hi, a_lo;
-              chunk((S::enc_first(l) && nact > 0 && nch > nact) ? (c == 0 ? nact : c - 1) : c, !sp, a_hi, a_lo);
-              for (int sub = 0; sub < 2; ++sub) STAGE(a_hi + (uint32_t)sub * 64);
-            }
-          }
-          if (PAIR) umma_commit_pair(BAR(BAR_DFULL + b));           // accumulator of layer g complete (in both CTAs)
-          else umma_commit(BAR(BAR_DFULL + b));
-        }
-      }
-    }
-  } else if (NET == NET_SPACE && !PAIR && (warp == 2 || warp == 3)) {
+  } else if (NET == NET_SPACE && (warp == 2 || warp == 3)) {
     // =============================== compositing warps (coarse-pass fusion) ===============================
     if (P.fuse.on) {
-      float* cdf = reinterpret_cast<float*>(smem + S::misc_base + MISC_CDF) + (warp - 2) * 64;
-      if (P.fuse.n2 <= 128) fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL), BAR(BAR_RAWEMPTY), n_tiles, warp - 2, lane, WSHARE);
-      else fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL), BAR(BAR_RAWEMPTY), n_tiles, warp - 2, lane, WSHARE);
+      const int j = warp - 2;
+      float* cdf = reinterpret_cast<float*>(smem + S::misc_base + MISC_CDF) + j * 64;
+      if (P.fuse.n2 <= 128)
+        fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane, false);
+      else
+        fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane, false);
     }
-  } else if (warp >= S::EPI_W0) {
-    // =============================== encoding + epilogue warps ===============================
-    const int ew = warp - S::EPI_W0;            // 0..7
-    const int q = warp & 3, hh = ew >> 2;       // TMEM lane quarter (fixed by the warp id), column half / encoding half
-    const int row = q * 32 + lane;
-    const uint32_t lane_taddr = tmem_base + ((uint32_t)(q * 32) << 16);
+  } else if (wgi >= MATH_WG0) {
+    // =============================== math warpgroups: encoding, MMAs, epilogues ===============================
+    const int wg = wgi - MATH_WG0;                    // 0, 1: rows 64 wg .. 64 wg + 63 of every tile
+    const int wt = tid & 127;
+    const int erow = wg * 64 + (wt & 63), ehalf = wt >> 6;    // encoding: two threads per row, one per half of the frequencies
+    const int r0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2);    // accumulator fragment: rows r0, r0 + 8, columns 8 j + cq, +1
+    const int cq = 2 * (lane & 3);
+    const uint32_t a_row = (uint32_t)wg * 8u * 1024u;         // byte offset of the warpgroup's rows in a swizzled block
     const float* bias_all = P.aux + AUX_BIAS;
     const bool lerp = (NET == NET_MOTION) && (P.lerp_force >= 0 ? (P.lerp_force != 0) : (P.lerp_flag && *P.lerp_flag != 0));
-    uint32_t g = 0;
-#ifdef STNERF_TIMING
-    EpiTiming tm;
-    const long long t_begin = clock64();
-#endif
-
-    // encoding of the first tile
-    Pt cur = fetch_pt(P.src, (long long)blockIdx.x * TILE_M + row, n_points);
-    float carry[2] = {0.f, 0.f};
-    // zero padding of the MotionNet encoding blocks (chunks 5.. of block 1, 6.. of block 0): written once when the encoding has
-    // its own blocks, before every tile when it shares them with the activations
-    auto zero_motion_pads = [&]() {
-      uint8_t* enc = smem + S::enc_base + hh * ABLOCK;
-      for (int c = (hh == 0 ? 48 : 40); c < 64; c += 8) {
-        const uint32_t off = sw128_offset(row, c);
-        *reinterpret_cast<uint4*>(enc + off) = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4*>(enc + S::ENC_LO_STRIDE + off) = make_uint4(0, 0, 0, 0);
-      }
-    };
-    if (NET == NET_MOTION) zero_motion_pads();
-    // arrive on the leader's barrier `i` (this CTA's own barrier outside pair mode)
-    auto ARRIVE = [&](int i) { if (PAIR) mbar_arrive_cluster(LBAR(i)); else mbar_arrive(BAR(i)); };
-    if (in_range((long long)blockIdx.x)) {
-      encode_piece<NET, 0>(smem, cur, row, hh, exact, lerp, carry);
-      encode_piece<NET, 1>(smem, cur, row, hh, exact, lerp, carry);
-      if (NET == NET_MOTION) encode_piece<NET, 2>(smem, cur, row, hh, exact, lerp, carry);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) ARRIVE(BAR_AREADY + AREADY_ENC);
-    }
-    uint32_t tile_no = 0;                       // tiles this CTA has finished (phase of the fused compositing hand-off)
-    for (long long tile = blockIdx.x; in_range(tile); tile += gridDim.x, ++tile_no) {
-      const long long nt = tile + gridDim.x;
-      const bool have_next = in_range(nt);
-      Pt nxt = cur;
-      float sig_dot = 0.f;
-      for (int l = 0; l < S::N_LAYERS; ++l, ++g) {
-        const uint32_t b = g & 1;
-        const bool last = (l == S::N_LAYERS - 1);
-        const int width = S::n_out(l);
-        const float* bias = bias_all + l * 256;
-        const uint32_t dcol = lane_taddr + b * S::d_stride;
-        if (!last) {
-          TSTAMP(tw0);
-          mbar_wait(BAR(BAR_DFULL + b), (g >> 1) & 1);
-          tc_fence_after();
-#ifdef STNERF_TIMING
-          tm.wait_dfull += clock64() - tw0;
-#endif
-          const int nchunk = width / 64;
-          if (NET == NET_SPACE && l == 6) {
-            for (int j = 0; j < nchunk; ++j)
-              sig_dot = epi_hidden_chunk<true, PAIR, ATMEM>(dcol, j, hh, row, bias, P.aux + AUX_WSIG, smem + S::act_base + j * ABLOCK,
-                                                     S::LO_STRIDE, split(l + 1), lane, LBAR(BAR_AREADY + 2 * j), sig_dot
-#ifdef STNERF_TIMING
-                                               , tm
-#endif
-              );
-          } else {
-            for (int j = 0; j < nchunk; ++j)
-              epi_hidden_chunk<false, PAIR, ATMEM>(dcol, j, hh, row, bias, nullptr, smem + S::act_base + j * ABLOCK, S::LO_STRIDE, split(l + 1),
-                                            lane, LBAR(BAR_AREADY + 2 * j), 0.f
-#ifdef STNERF_TIMING
-                                      , tm
-#endif
-              );
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) ARRIVE(BAR_DEMPTY + b);
-          // Idle time until the next accumulator is ready: fetch and encode the NEXT tile's points piece by piece.
-          // The encoding buffer is free once the MMAs of layer ENC_LAST_USE are done (observed through d_full above).
-          //   SpaceNet : fetch after layer 1, pieces after layers 4 and 5
-          //   MotionNet: fetch after layer 0, pieces after layers 1, 2, 3
-          if (have_next) {
-            TSTAMP(te0);
-            constexpr int L_FETCH = (NET == NET_SPACE) ? 1 : 0;
-            constexpr int L_P0 = (NET == NET_SPACE) ? 4 : 1;
-            if (l == L_FETCH) nxt = fetch_pt(P.src, nt * TILE_M + row, n_points);
-            if (!S::ENC_ALIASES_ACT) {
-              if (l == L_P0) encode_piece<NET, 0>(smem, nxt, row, hh, exact, lerp, carry);
-              if (l == L_P0 + 1) encode_piece<NET, 1>(smem, nxt, row, hh, exact, lerp, carry);
-              if (NET == NET_MOTION && l == L_P0 + 2) encode_piece<NET, 2>(smem, nxt, row, hh, exact, lerp, carry);
-              if (l == L_P0 + (NET == NET_SPACE ? 1 : 2)) {
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) ARRIVE(BAR_AREADY + AREADY_ENC);
-              }
-            }
-#ifdef STNERF_TIMING
-            tm.enc += clock64() - te0;
-#endif
-          }
-        } else {
-          // last layer: 128 features -> 3-wide head in fp32 (rgb_net.3 / motion_net.10).
-          // SpaceNet: the bias is the per-ray vector of head_bias_kernel (dir/time part of rgb_net.1 + b1).
-          const float* brow = (NET == NET_SPACE) ? (P.cbuf + (size_t)cur.cidx * 128) : bias;
-          TSTAMP(tl0);
-          float4 bb4[8];                                           // per-ray bias row: L2-resident, fetched ahead of the wait
-          {
-            const float4* bp = reinterpret_cast<const float4*>(brow + hh * 32);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) bb4[i] = __ldg(bp + i);
-          }
-          mbar_wait(BAR(BAR_DFULL + b), (g >> 1) & 1);
-          tc_fence_after();
-          TSTAMP(tl1);
-          float dot3[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            uint32_t acc[32];
-            const int col0 = j * 64 + hh * 32;
-            tmem_ld32_issue(dcol + (uint32_t)col0, acc);
-            float4 bn4[8];
-            if (j == 0) {
-              const float4* bp = reinterpret_cast<const float4*>(brow + 64 + hh * 32);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) bn4[i] = __ldg(bp + i);
-            }
-            tmem_ld_wait(acc);
-            float v[32];
-#pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              const float4 bb = bb4[c >> 2];
-              const float bc = (c & 3) == 0 ? bb.x : (c & 3) == 1 ? bb.y : (c & 3) == 2 ? bb.z : bb.w;
-              v[c] = fmaxf(__uint_as_float(acc[c]) + bc, 0.f);
-            }
-#pragma unroll
-            for (int o = 0; o < 3; ++o) {
-              const float4* wp = reinterpret_cast<const float4*>(P.aux + AUX_WOUT + o * 128 + col0);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 ww = __ldg(wp + i);
-                dot3[o] = fmaf(v[4 * i], ww.x, dot3[o]);
-                dot3[o] = fmaf(v[4 * i + 1], ww.y, dot3[o]);
-                dot3[o] = fmaf(v[4 * i + 2], ww.z, dot3[o]);
-                dot3[o] = fmaf(v[4 * i + 3], ww.w, dot3[o]);
-              }
-            }
-            if (j == 0) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) bb4[i] = bn4[i];
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) ARRIVE(BAR_DEMPTY + b);
-          if (S::ENC_ALIASES_ACT && have_next) {
-            // The last layer's MMAs have retired (d_full above), so nothing reads the activation blocks any more: the next
-            // tile's encoding goes into them now, and its layer 0 runs while this tile's head is combined and written out.
-            zero_motion_pads();
-            encode_piece<NET, 0>(smem, nxt, row, hh, exact, lerp, carry);
-            encode_piece<NET, 1>(smem, nxt, row, hh, exact, lerp, carry);
-            if (NET == NET_MOTION) encode_piece<NET, 2>(smem, nxt, row, hh, exact, lerp, carry);
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) ARRIVE(BAR_AREADY + AREADY_ENC);
-          }
-          // combine the two column halves through shared memory.  With the coarse-pass fusion the tile's FINAL rows go to
-          // `s_part` for the compositing warps, so the half sums travel through the first activation block instead: every
-          // MMA of this tile has retired (d_full above) and the next writer of that block is this very warp group (layer-0
-          // epilogue of the next tile).
-          const bool fused = (NET == NET_SPACE) && !PAIR && P.fuse.on;
-          float* s_half = fused ? reinterpret_cast<float*>(smem + S::scratch_base) : s_part;
-          if (hh == 1) {
-            s_half[row * 4 + 0] = dot3[0]; s_half[row * 4 + 1] = dot3[1]; s_half[row * 4 + 2] = dot3[2];
-            s_half[row * 4 + 3] = sig_dot;
-          }
-          epi_bar_sync();
-          if (fused && hh == 0) {
-            // the compositing warps must be done with the previous tile's rows (they have had a whole tile period)
-            if (tile_no > 0) mbar_wait(BAR(BAR_RAWEMPTY), (tile_no - 1) & 1);
-            const float o0 = dot3[0] + s_half[row * 4 + 0] + P.aux[AUX_BOUT + 0];
-            const float o1 = dot3[1] + s_half[row * 4 + 1] + P.aux[AUX_BOUT + 1];
-            const float o2 = dot3[2] + s_half[row * 4 + 2] + P.aux[AUX_BOUT + 2];
-            const float sg = sig_dot + s_half[row * 4 + 3] + P.aux[AUX_BSIG];
-            reinterpret_cast<float4*>(s_part)[row] = make_float4(o0, o1, o2, sg);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(BAR(BAR_RAWFULL));
-          }
-          if (hh == 0 && cur.out_index >= 0) {
-            const float o0 = dot3[0] + s_half[row * 4 + 0] + P.aux[AUX_BOUT + 0];
-            const float o1 = dot3[1] + s_half[row * 4 + 1] + P.aux[AUX_BOUT + 1];
-            const float o2 = dot3[2] + s_half[row * 4 + 2] + P.aux[AUX_BOUT + 2];
-            const int oi = cur.out_index;
-            if (NET == NET_SPACE) {
-              const float sg = sig_dot + s_half[row * 4 + 3] + P.aux[AUX_BSIG];
-              if (P.raw) reinterpret_cast<float4*>(P.raw)[oi] = make_float4(o0, o1, o2, sg);
-              if (P.rgb_out) { P.rgb_out[3 * (size_t)oi] = o0; P.rgb_out[3 * (size_t)oi + 1] = o1; P.rgb_out[3 * (size_t)oi + 2] = o2; }
-              if (P.sigma_out) P.sigma_out[oi] = sg;
-            } else {
-              const long long p = tile * TILE_M + row;          // compact point index
-              if (P.flow_out) { P.flow_out[3 * p] = o0; P.flow_out[3 * p + 1] = o1; P.flow_out[3 * p + 2] = o2; }
-              if (P.xyz_out) {                                  // layered_rfrender.py:356 / :510
-                P.xyz_out[3 * p] = __fadd_rn(cur.x, o0);
-                P.xyz_out[3 * p + 1] = __fadd_rn(cur.y, o1);
-                P.xyz_out[3 * p + 2] = __fadd_rn(cur.z, o2);
-              }
-            }
-          }
-          epi_bar_sync();       // the half sums are rewritten by the next tile
-#ifdef STNERF_TIMING
-          tm.last_wait += tl1 - tl0; tm.last_epi += clock64() - tl1; tm.tiles += 1;
-#endif
+    const bool fused = (NET == NET_SPACE) && P.fuse.on;
+    uint32_t cnt = 0, tile_no = 0;
+    float acc[128];
+    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_no) {
+      // the previous tile's MMAs have retired in every warp of the warpgroup and its rows are written out: its blocks are free
+      wg_bar_sync(wg);
+      const Pt cur = fetch_pt(P.src, tile * TILE_M + erow, n_points);
+      if (ehalf == 0) s_rows[erow] = cur;
+      float carry[2] = {0.f, 0.f};
+      if (NET == NET_MOTION) {
+        // zero padding of the MotionNet encoding blocks (chunks 6.. of block 0, 5.. of block 1): the activations overwrite them
+        uint8_t* enc = smem + S::enc_base + ehalf * ABLOCK;
+        for (int c = (ehalf == 0 ? 48 : 40); c < 64; c += 8) {
+          const uint32_t off = sw128_offset(erow, c);
+          *reinterpret_cast<uint4*>(enc + off) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(enc + S::ENC_LO_STRIDE + off) = make_uint4(0, 0, 0, 0);
         }
       }
-      cur = nxt;
+      encode_piece<NET, 0>(smem, cur, erow, ehalf, exact, lerp, carry);
+      encode_piece<NET, 1>(smem, cur, erow, ehalf, exact, lerp, carry);
+      if (NET == NET_MOTION) encode_piece<NET, 2>(smem, cur, erow, ehalf, exact, lerp, carry);
+      float sig0 = 0.f, sig1 = 0.f;
+      for (int l = 0; l < S::N_LAYERS; ++l) {
+        // the A operand of this layer (encoding / previous epilogue) is written by every thread of the warpgroup
+        fence_proxy_async();
+        wg_bar_sync(wg);
+        const bool last = (l == S::N_LAYERS - 1);
+        if (!last) {
+          mma_layer<NET, (NET == NET_SPACE ? 256 : 128), LOFIRST>(acc, l, split(l), sbase, a_row, bars, cnt, lane);
+          if (NET == NET_SPACE && l == 6)
+            epi_hidden<NET, 256, true>(acc, bias_all + l * 256, P.aux + AUX_WSIG, smem, r0, cq, split(l + 1), sig0, sig1);
+          else
+            epi_hidden<NET, (NET == NET_SPACE ? 256 : 128), false>(acc, bias_all + l * 256, nullptr, smem, r0, cq, split(l + 1), sig0, sig1);
+          continue;
+        }
+        // last layer: 128 features -> 3-wide head in fp32 (rgb_net.3 / motion_net.10).
+        // SpaceNet: the bias is the per-ray vector of head_bias_kernel (dir/time part of rgb_net.1 + b1).
+        mma_layer<NET, 128, LOFIRST>(acc, l, split(l), sbase, a_row, bars, cnt, lane);
+        const Pt p0 = s_rows[r0], p1 = s_rows[r0 + 8];
+        const float* b0 = (NET == NET_SPACE) ? (P.cbuf + (size_t)p0.cidx * 128) : bias_all + l * 256;
+        const float* b1 = (NET == NET_SPACE) ? (P.cbuf + (size_t)p1.cidx * 128) : bias_all + l * 256;
+        float d0[3] = {0.f, 0.f, 0.f}, d1[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = 8 * j + cq;
+          const float2 ba = __ldg(reinterpret_cast<const float2*>(b0 + col));
+          const float2 bb = __ldg(reinterpret_cast<const float2*>(b1 + col));
+          const float v00 = fmaxf(acc[4 * j] + ba.x, 0.f), v01 = fmaxf(acc[4 * j + 1] + ba.y, 0.f);
+          const float v10 = fmaxf(acc[4 * j + 2] + bb.x, 0.f), v11 = fmaxf(acc[4 * j + 3] + bb.y, 0.f);
+#pragma unroll
+          for (int o = 0; o < 3; ++o) {
+            const float2 w = __ldg(reinterpret_cast<const float2*>(P.aux + AUX_WOUT + o * 128 + col));
+            d0[o] = fmaf(v00, w.x, d0[o]); d0[o] = fmaf(v01, w.y, d0[o]);
+            d1[o] = fmaf(v10, w.x, d1[o]); d1[o] = fmaf(v11, w.y, d1[o]);
+          }
+        }
+#pragma unroll
+        for (int o = 0; o < 3; ++o) { d0[o] = quad_sum(d0[o]) + P.aux[AUX_BOUT + o]; d1[o] = quad_sum(d1[o]) + P.aux[AUX_BOUT + o]; }
+        if (NET == NET_SPACE) { sig0 = quad_sum(sig0) + P.aux[AUX_BSIG]; sig1 = quad_sum(sig1) + P.aux[AUX_BSIG]; }
+        if (fused) {
+          // the compositing warp of these rows must be done with the previous tile's (it has had a whole tile period)
+          if (tile_no > 0) mbar_wait(BAR(BAR_RAWEMPTY + wg), (tile_no - 1) & 1);
+          if ((lane & 3) == 0) {
+            reinterpret_cast<float4*>(s_part)[r0] = make_float4(d0[0], d0[1], d0[2], sig0);
+            reinterpret_cast<float4*>(s_part)[r0 + 8] = make_float4(d1[0], d1[1], d1[2], sig1);
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(BAR(BAR_RAWFULL + wg));
+        }
+        if ((lane & 3) == 0) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const Pt& p = h ? p1 : p0;
+            const float* o = h ? d1 : d0;
+            const float sg = h ? sig1 : sig0;
+            if (p.out_index < 0) continue;
+            const int oi = p.out_index;
+            if (NET == NET_SPACE) {
+              if (P.raw) reinterpret_cast<float4*>(P.raw)[oi] = make_float4(o[0], o[1], o[2], sg);
+              if (P.rgb_out) { P.rgb_out[3 * (size_t)oi] = o[0]; P.rgb_out[3 * (size_t)oi + 1] = o[1]; P.rgb_out[3 * (size_t)oi + 2] = o[2]; }
+              if (P.sigma_out) P.sigma_out[oi] = sg;
+            } else {
+              const long long pidx = tile * TILE_M + r0 + 8 * h;     // compact point index
+              if (P.flow_out) { P.flow_out[3 * pidx] = o[0]; P.flow_out[3 * pidx + 1] = o[1]; P.flow_out[3 * pidx + 2] = o[2]; }
+              if (P.xyz_out) {                                       // layered_rfrender.py:356 / :510
+                P.xyz_out[3 * pidx] = __fadd_rn(p.x, o[0]);
+                P.xyz_out[3 * pidx + 1] = __fadd_rn(p.y, o[1]);
+                P.xyz_out[3 * pidx + 2] = __fadd_rn(p.z, o[2]);
+              }
+            }
+          }
+        }
+      }
     }
-#ifdef STNERF_TIMING
-    if (blockIdx.x == 0 && lane == 0 && tm.n > 0)
-      printf("[timing net %d warp %d] chunks %lld | per chunk: ld %lld math %lld fence %lld arrive %lld | d_full wait per layer %lld | total cycles %lld\n",
-             NET, warp, tm.n, tm.ld / tm.n, tm.math / tm.n, tm.fence / tm.n, tm.arrive / tm.n, tm.wait_dfull * 4 / tm.n, clock64() - t_begin);
-    if (blockIdx.x == 0 && lane == 0 && tm.tiles > 0 && warp == 4)
-      printf("[timing net %d] tiles %lld | per tile: encode %lld, last-layer wait %lld, last-layer epilogue %lld, total %lld\n", NET, tm.tiles,
-             tm.enc / tm.tiles, tm.last_wait / tm.tiles, tm.last_epi / tm.tiles, (clock64() - t_begin) / tm.tiles);
-#endif
   }
-  // teardown
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR || WSHARE) cluster_sync_all();        // neither CTA leaves (or frees tensor memory) while the other may still touch it
-  if (warp == 1) { if (PAIR) tmem_dealloc_pair(tmem_base, S::tmem_cols); else tmem_dealloc(tmem_base, S::tmem_cols); }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1599,156 +888,59 @@ __global__ void __launch_bounds__(128) head_bias_kernel(PointSrc src, const floa
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// self-test: 128 x N x 64 fp16 UMMA (N = 256) through exactly the descriptors / swizzles / bulk copy / TMEM load used above
+// self-test: D (128 x 256) = A (128 x 64) * B^T (256 x 64) in fp16 through exactly the descriptors / swizzles / bulk copy /
+// accumulator fragment of the kernel above (two math warpgroups of 64 rows each)
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const float* __restrict__ A, const uint8_t* __restrict__ Bstages,
-                                                              float* __restrict__ D, int reps, int ts) {
-  // ts != 0: the A operand goes through TENSOR memory in the layout of the SpaceNet epilogue (SPACE_A_TMEM): per K=16 step 8 columns
-  // of packed fp16 pairs at a 16-column pitch, written with tcgen05.st, read by tcgen05.mma [d], [a], b-desc
+__global__ void __launch_bounds__(256, 1) wgmma_selftest_kernel(const float* __restrict__ A, const uint8_t* __restrict__ Bstages,
+                                                               float* __restrict__ D, int reps) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar = sbase + ABLOCK + 2 * STAGE_BYTES, bar2 = bar + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + ABLOCK + 2 * STAGE_BYTES + 16);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t bar = sbase + ABLOCK + 2 * STAGE_BYTES;
+  const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127, lane = tid & 31;
   if ((sbase & 1023u) != 0) __trap();
   if (tid == 0) {
     mbar_init(bar, 1);
-    mbar_init(bar2, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) tmem_alloc(smem_u32(tmem_slot), 512);
-  // A: row `tid`, 64 columns, written with the epilogue's store path (hi only)
-  for (int c0 = 0; c0 < 64; c0 += 32) {
-    float v[32];
-    for (int i = 0; i < 32; ++i) v[i] = A[tid * 64 + c0 + i];
-    store_row_split<32>(smem, 0, tid, c0, v, false);
+  if (tid < 128) {                               // A: row `tid`, 64 columns, written with the encoder's store path (hi only)
+    for (int c0 = 0; c0 < 64; c0 += 32) {
+      float v[32];
+      for (int i = 0; i < 32; ++i) v[i] = A[tid * 64 + c0 + i];
+      store_row_split<32>(smem, 0, tid, c0, v, false);
+    }
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (ts) {
-    for (int k4 = 0; k4 < 4; ++k4) {
-      uint32_t hp[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) hp[e] = pack_f16x2(A[tid * 64 + k4 * 16 + 2 * e], A[tid * 64 + k4 * 16 + 2 * e + 1]);
-      tmem_st8(tmem_base + ((uint32_t)(warp * 32) << 16) + 256u + 16u * k4, hp);
-    }
-    tmem_st_wait();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-  }
-  if (tid == 0 && ts) {
-    mbar_expect_tx(bar2, 2 * STAGE_BYTES);
-    bulk_g2s(sbase + ABLOCK, Bstages, 2 * STAGE_BYTES, bar2);
-    mbar_wait(bar2, 0);
-    tc_fence_after();
-    for (int rep = 0; rep < reps; ++rep)
-      for (int sub = 0; sub < 2; ++sub)
-        for (int ks = 0; ks < 2; ++ks)
-          umma_f16_ts(tmem_base, tmem_base + 256u + 32u * sub + 16u * ks,
-                      make_desc_sw64(sbase + ABLOCK + sub * STAGE_BYTES + ks * 32), idesc_n(256), (rep | sub | ks) ? 1u : 0u);
-    umma_commit(bar);
-  } else if (tid == 0) {
-    mbar_expect_tx(bar2, 2 * STAGE_BYTES);                       // two 32-wide k sub-chunks
-    bulk_g2s(sbase + ABLOCK, Bstages, 2 * STAGE_BYTES, bar2);
-    mbar_wait(bar2, 0);
-    tc_fence_after();
-    for (int rep = 0; rep < reps; ++rep)       // reps > 1: the same product accumulated again and again (accumulation probe)
-      for (int sub = 0; sub < 2; ++sub)
-        for (int ks = 0; ks < 2; ++ks)
-          umma_f16(tmem_base, make_desc_sw128(sbase + sub * 64 + ks * 32),
-                   make_desc_sw64(sbase + ABLOCK + sub * STAGE_BYTES + ks * 32), idesc_n(256), (rep | sub | ks) ? 1u : 0u);
-    umma_commit(bar);
+  if (tid == 0) {
+    mbar_expect_tx(bar, 2 * STAGE_BYTES);        // two 32-wide k sub-chunks
+    bulk_g2s(sbase + ABLOCK, Bstages, 2 * STAGE_BYTES, bar);
   }
   mbar_wait(bar, 0);
-  tc_fence_after();
-  for (int j = 0; j < 8; ++j) {
-    uint32_t acc[32];
-    tmem_ld32_issue(tmem_base + ((uint32_t)(warp * 32) << 16) + j * 32, acc);
-    tmem_ld_wait(acc);
+  float acc[128];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) D[(warp * 32 + lane) * 256 + j * 32 + i] = __uint_as_float(acc[i]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 512);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// self-test of the CTA-pair protocol: D (256 x 256) = A (256 x 64) * B^T (256 x 64) with ONE cta_group::2 accumulator.
-// CTA r of the cluster holds A rows [128 r, 128 r + 128) and B rows (= output columns) [128 r, 128 r + 128) of every stage;
-// the leader waits for its own bulk copy, for the peer's (relayed by a remote arrive) and for both A tiles, issues the
-// MMAs and commits to the `done` barrier of both CTAs; each CTA reads its 128 accumulator rows.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int PAIR_HALF_STAGE = STAGE_BYTES / 2;
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128, 1)
-umma_pair_selftest_kernel(const float* __restrict__ A, const uint8_t* __restrict__ Bstages, float* __restrict__ D) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t rank = cluster_ctarank();
-  const uint32_t bars = sbase + ABLOCK + 2 * PAIR_HALF_STAGE;
-  const uint32_t bar_full = bars, bar_peer = bars + 8, bar_a = bars + 16, bar_done = bars + 24;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + ABLOCK + 2 * PAIR_HALF_STAGE + 32);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if ((sbase & 1023u) != 0) __trap();
-  if (tid == 0) {
-    mbar_init(bar_full, 1);
-    mbar_init(bar_peer, 1);
-    mbar_init(bar_a, 2);
-    mbar_init(bar_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc_pair(smem_u32(tmem_slot), 256);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                          // barriers of both CTAs initialised before any remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  for (int c0 = 0; c0 < 64; c0 += 32) {        // this CTA's 128 rows of A through the epilogue's store path (hi only)
-    float v[32];
-    for (int i = 0; i < 32; ++i) v[i] = A[((int)rank * 128 + tid) * 64 + c0 + i];
-    store_row_split<32>(smem, 0, tid, c0, v, false);
-  }
-  // exactly the hand-off of the MLP kernel: generic-proxy stores -> async-proxy fence -> CTA barrier -> one release-arrive
-  // (cluster scope) on the LEADER's barrier; the leader's acquire-wait orders the peer's tile before its MMAs
-  fence_proxy_async();
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_cluster(map_to_cta(bar_a, 0));
-    mbar_expect_tx(bar_full, 2 * PAIR_HALF_STAGE);
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  acc_fence<128>(acc);
+  wgmma_fence();
+  for (int rep = 0; rep < reps; ++rep) {         // reps > 1: the same product accumulated again and again (accumulation probe)
+#pragma unroll
     for (int sub = 0; sub < 2; ++sub)
-      bulk_g2s(sbase + ABLOCK + sub * PAIR_HALF_STAGE, Bstages + (size_t)sub * STAGE_BYTES + (size_t)rank * PAIR_HALF_STAGE,
-               PAIR_HALF_STAGE, bar_full);
-    mbar_wait(bar_full, 0);
-    if (rank == 1) {
-      mbar_arrive_cluster(map_to_cta(bar_peer, 0));               // relay: the peer's half of B has landed
-    } else {
-      mbar_wait_cluster(bar_peer, 0);
-      mbar_wait_cluster(bar_a, 0);
-      tc_fence_after();
-      for (int sub = 0; sub < 2; ++sub)
-        for (int ks = 0; ks < 2; ++ks)
-          umma_f16_pair(tmem_base, make_desc_sw128(sbase + sub * 64 + ks * 32),
-                        make_desc_sw64(sbase + ABLOCK + sub * PAIR_HALF_STAGE + ks * 32), idesc_pair_n(256), (sub | ks) ? 1u : 0u);
-      umma_commit_pair(bar_done);
-    }
-  }
-  mbar_wait(bar_done, 0);
-  tc_fence_after();
-  for (int j = 0; j < 8; ++j) {
-    uint32_t acc[32];
-    tmem_ld32_issue(tmem_base + ((uint32_t)(warp * 32) << 16) + j * 32, acc);
-    tmem_ld_wait(acc);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) D[((int)rank * 128 + warp * 32 + lane) * 256 + j * 32 + i] = __uint_as_float(acc[i]);
+      for (int ks = 0; ks < 2; ++ks)
+        wgmma_n256(acc, desc_sw128(sbase + (uint32_t)wg * 8192u + sub * 64 + ks * 32),
+                   desc_sw64(sbase + ABLOCK + sub * STAGE_BYTES + ks * 32));
+    wgmma_commit();
+    wgmma_wait<0>();
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                          // both CTAs are done with the accumulator before either frees it
-  if (warp == 0) tmem_dealloc_pair(tmem_base, 256);
+  acc_fence<128>(acc);
+  const int r0 = wg * 64 + (wt >> 5) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int col = 8 * j + cq;
+    D[r0 * 256 + col] = acc[4 * j];
+    D[r0 * 256 + col + 1] = acc[4 * j + 1];
+    D[(r0 + 8) * 256 + col] = acc[4 * j + 2];
+    D[(r0 + 8) * 256 + col + 1] = acc[4 * j + 3];
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1913,11 +1105,13 @@ int tc_pack_motionnet(TcNet& net, const float* p) {
   return pack_stream(net, layers, aux, stream_bytes_per_tile<NET_MOTION>());
 }
 
+
 // D = A * B^T for random A (128x64, rounded to fp16), B (256x64) through the tensor-core path; max |D - reference|.
-// reps > 1 (accumulation probe): all-positive operands, the product accumulated `reps` times into the same TMEM accumulator
+// reps > 1 (accumulation probe): all-positive operands, the product accumulated `reps` times into the same register accumulator
 // (4*reps MMAs of K=16); reports the max and the MEAN SIGNED relative error against the fp64 sum -- a negative mean that grows
 // with reps is the signature of round-toward-zero accumulation inside the tensor core.
-int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host, int ts) {
+int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host) {
+  if (reps < 1) return STNERF_EINVAL;
   std::vector<float> Af(128 * 64), Bf(256 * 64);
   uint32_t s = 12345u;
   const bool probe = reps > 1;
@@ -1938,8 +1132,8 @@ int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host
   STNERF_CUDA(cudaMemcpy(dA, Af.data(), Af.size() * 4, cudaMemcpyHostToDevice));
   STNERF_CUDA(cudaMemcpy(dB, stages.data(), stages.size(), cudaMemcpyHostToDevice));
   const int smem = ABLOCK + 2 * STAGE_BYTES + 64;
-  STNERF_CUDA(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  umma_selftest_kernel<<<1, 128, smem>>>(dA, dB, dD, reps, ts);
+  STNERF_CUDA(cudaFuncSetAttribute(wgmma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  wgmma_selftest_kernel<<<1, 256, smem>>>(dA, dB, dD, reps);
   STNERF_LAUNCH_CHECK();
   STNERF_CUDA(cudaDeviceSynchronize());
   std::vector<float> D(128 * 256);
@@ -1959,71 +1153,15 @@ int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host
   if (mean_signed_rel_host) *mean_signed_rel_host = (float)(signed_rel / (128.0 * 256.0));
   return STNERF_OK;
 }
-int tc_selftest(float* max_err_host) { return tc_selftest_accum(1, max_err_host, nullptr, 0); }
-int tc_selftest_ts(float* max_err_host) { return tc_selftest_accum(1, max_err_host, nullptr, 1); }
-
-// The same for the CTA-pair protocol: 256 x 256 x 64.
-int tc_selftest_pair(float* max_err_host) {
-  std::vector<float> Af(256 * 64), Bf(256 * 64);
-  uint32_t s = 777u;
-  auto rnd = [&s]() { s = s * 1664525u + 1013904223u; return ((s >> 8) & 0xFFFF) / 65536.0f - 0.5f; };
-  for (auto& v : Af) v = __half2float(__float2half_rn(rnd()));
-  for (auto& v : Bf) v = __half2float(__float2half_rn(rnd()));
-  std::vector<uint8_t> stages(2 * STAGE_BYTES, 0);
-  for (int sub = 0; sub < 2; ++sub)
-    for (int n = 0; n < 256; ++n)
-      for (int c = 0; c < 32; ++c) {
-        const __half h = __float2half_rn(Bf[n * 64 + sub * 32 + c]);
-        memcpy(stages.data() + sub * STAGE_BYTES + sw64_offset(n, c), &h, 2);
-      }
-  float *dA = nullptr, *dD = nullptr; uint8_t* dB = nullptr;
-  STNERF_CUDA(cudaMalloc((void**)&dA, Af.size() * 4));
-  STNERF_CUDA(cudaMalloc((void**)&dB, stages.size()));
-  STNERF_CUDA(cudaMalloc((void**)&dD, 256 * 256 * 4));
-  STNERF_CUDA(cudaMemset(dD, 0, 256 * 256 * 4));
-  STNERF_CUDA(cudaMemcpy(dA, Af.data(), Af.size() * 4, cudaMemcpyHostToDevice));
-  STNERF_CUDA(cudaMemcpy(dB, stages.data(), stages.size(), cudaMemcpyHostToDevice));
-  const int smem = ABLOCK + 2 * PAIR_HALF_STAGE + 64;
-  STNERF_CUDA(cudaFuncSetAttribute(umma_pair_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  umma_pair_selftest_kernel<<<2, 128, smem>>>(dA, dB, dD);
-  STNERF_LAUNCH_CHECK();
-  STNERF_CUDA(cudaDeviceSynchronize());
-  std::vector<float> D(256 * 256);
-  STNERF_CUDA(cudaMemcpy(D.data(), dD, D.size() * 4, cudaMemcpyDeviceToHost));
-  cudaFree(dA); cudaFree(dB); cudaFree(dD);
-  float worst = 0.f;
-  for (int m = 0; m < 256; ++m)
-    for (int n = 0; n < 256; ++n) {
-      double ref = 0;
-      for (int k = 0; k < 64; ++k) ref += (double)Af[m * 64 + k] * Bf[n * 64 + k];
-      worst = fmaxf(worst, fabsf((float)ref - D[m * 256 + n]));
-    }
-  *max_err_host = worst;
-  return STNERF_OK;
-}
+int tc_selftest(float* max_err_host) { return tc_selftest_accum(1, max_err_host, nullptr); }
 
 template <int NET, bool LOFIRST>
 static int launch_tc_variant(const TcParams& P, int num_sms, cudaStream_t st) {
   // per-device attribute, set on every launch (one process may drive several devices; cost: microseconds)
   using S = Sched<NET>;
-  constexpr bool PAIR = (NET == NET_SPACE) && (SPACE_CTA_PAIR != 0);
-  constexpr bool WSHARE = (NET == NET_SPACE) && (SPACE_WSHARE != 0) && !PAIR;      // (an odd SM count leaves one SM idle: 148 is even)
-  auto kern = mlp_tc_kernel<NET, PAIR, WSHARE, LOFIRST>;
+  auto kern = mlp_tc_kernel<NET, LOFIRST>;
   STNERF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::smem_total));
-  if (S::CTAS_PER_SM > 1)     // ask for the largest shared-memory carveout, or the second CTA does not fit next to the first
-    STNERF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  if (PAIR || WSHARE) {       // clusters of two CTAs (one TPC): grid = an even number of CTAs, one per SM
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(num_sms & ~1)); cfg.blockDim = dim3(S::N_THREADS); cfg.dynamicSmemBytes = S::smem_total; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    STNERF_CUDA(cudaLaunchKernelEx(&cfg, kern, P));
-    ++g_launches;
-    return STNERF_OK;
-  }
-  kern<<<num_sms * S::CTAS_PER_SM, S::N_THREADS, S::smem_total, st>>>(P);
+  kern<<<num_sms, NTHREADS, S::smem_total, st>>>(P);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
 }
@@ -2033,7 +1171,7 @@ static int launch_tc(const TcParams& P, int num_sms, cudaStream_t st) {
   return P.lo_first ? launch_tc_variant<NET, true>(P, num_sms, st) : launch_tc_variant<NET, false>(P, num_sms, st);
 }
 
-bool tc_can_fuse_coarse(int n1, int n2) { return SPACE_CTA_PAIR == 0 && n1 == 64 && n2 >= 1 && n2 <= 256; }
+bool tc_can_fuse_coarse(int n1, int n2) { return n1 == 64 && n2 >= 1 && n2 <= 256; }
 
 int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW&, int precision, float* cbuf, float* raw,
                        float* rgb_out, float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse, int lo_first) {

@@ -1,11 +1,11 @@
-// tcgen05 (5th-gen tensor core) evaluation of SpaceNet / MotionNet: precision modes TC_3XF16 and TC_F16.
+// Warpgroup-MMA (sm_90a wgmma) evaluation of SpaceNet / MotionNet: precision modes TC_3XF16, TC_3XF16_CF, TC_MIXED and TC_F16.
 #pragma once
 #include "common.cuh"
 
 namespace stnerf {
 
 // Coarse-pass fusion (SURVEY 8a a10-a12 behind a8): with n1 = 64 a 128-point tile of the SpaceNet kernel is exactly two rays of
-// one layer, so the kernel's two spare warps composite the tile's (rgb, sigma) rows straight from shared memory
+// one layer, so the kernel's two compositing warps composite the tile's (rgb, sigma) rows straight from shared memory
 // (layers/render_layer.py:8-58), draw the n2 fine depths (utils/sample_pdf.py:18-63) and write sort(cat(t, z))
 // (modeling/layered_rfrender.py:459-463) -- the coarse rgb / sigma never leave the SM, and the work hides under the next
 // tile's MMAs.  Arithmetic: resample.cuh, shared with the stand-alone compositing kernel.
@@ -44,10 +44,8 @@ size_t tc_aux_floats();
 size_t tc_tail_floats(bool is_space);
 int tc_export(const TcNet& net, bool is_space, uint8_t* stream_host, float* aux_host, float* tail_host);
 int tc_import(TcNet& net, bool is_space, int use_time, const uint8_t* stream_host, const float* aux_host, const float* tail_host);
-int tc_selftest(float* max_err_host);   // one 128x128x64 UMMA vs a host reference
-int tc_selftest_ts(float* max_err_host);   // the same product with the A operand in tensor memory (tcgen05.st layout of the SpaceNet epilogue)
-int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host, int ts = 0);   // accumulation probe (see mlp_tc.cu)
-int tc_selftest_pair(float* max_err_host);   // 256x256x64 through one cta_group::2 accumulator (two CTAs of a cluster)
+int tc_selftest(float* max_err_host);   // one 128x256x64 warpgroup-MMA product vs a host reference
+int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host);   // accumulation probe (see mlp_tc.cu)
 int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW& w32, int precision, float* cbuf, float* raw,
                        float* rgb_out, float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse = nullptr,
                        int lo_first = 0);

@@ -1,4 +1,4 @@
-"""layers/RaySamplePoint.py of the reference on the B200 kernels (the module `demo/*.py` imports `RaySamplePoint` from)."""
+"""layers/RaySamplePoint.py of the reference on the native kernels (the module `demo/*.py` imports `RaySamplePoint` from)."""
 import torch
 
 from stnerf_b200 import ops

@@ -1,4 +1,4 @@
-"""Reference import name `layers` (layers/__init__.py:1-3): per-stage operators on the B200 kernels.
+"""Reference import name `layers` (layers/__init__.py:1-3): per-stage operators on the native kernels.
 
 Submodules that exist here (`RaySamplePoint`, `render_layer`, `loss`) replace the reference's; any other `layers.<name>`
 (e.g. `layers.camera_transform`) falls through to the reference tree when one is on sys.path (stnerf_b200/_fallthrough.py)."""

@@ -1,4 +1,4 @@
-"""layers/render_layer.py of the reference on the B200 compositing kernel."""
+"""layers/render_layer.py of the reference on the native compositing kernel."""
 import torch
 
 from stnerf_b200 import ops

@@ -1,4 +1,4 @@
-"""Reference import name `modeling` (modeling/__init__.py:3-7) backed by the B200 native renderer."""
+"""Reference import name `modeling` (modeling/__init__.py:3-7) backed by the native renderer."""
 from stnerf_b200.model import LayeredRFRender, build_layered_model
 
 # demo/walking_demo.py:18 imports `build_model`, which the reference package does not define; export it so the

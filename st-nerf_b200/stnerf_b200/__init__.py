@@ -1,4 +1,4 @@
-"""stnerf_b200 -- B200-native (sm_100a) implementation of the st-nerf layered ray-march hot path.
+"""stnerf_b200 -- H100-native (sm_90a) implementation of the st-nerf layered ray-march hot path.
 
 Python here is plumbing (device memory, streams, torch.distributed); the arithmetic lives in
 libstnerf_b200.so (st-nerf_b200/csrc, C ABI in include/stnerf.h).  The sibling packages `modeling`, `utils`,

@@ -15,7 +15,7 @@ PREC_FP32_SIMT, PREC_TC_3XF16, PREC_TC_F16, PREC_TC_MIXED, PREC_TC_3XF16_CF = 0,
 PRECISIONS = {"fp32": PREC_FP32_SIMT, "exact": PREC_TC_3XF16, "tc3": PREC_TC_3XF16, "fast": PREC_TC_F16, "mixed": PREC_TC_MIXED,
               "exact_cf": PREC_TC_3XF16_CF}
 
-# STNERF_B200_LIB selects an alternative build of the same ABI (A/B experiments: __graft_entry__.build_variant)
+# STNERF_B200_LIB selects another build of the same ABI (e.g. to compare two builds with scripts/dump_networks.py)
 LIB_PATH = os.environ.get("STNERF_B200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libstnerf_b200.so")
 
 
@@ -77,8 +77,6 @@ _SIGNATURES = {
     "stnerf_launch_count": (C.c_uint64, []),
     "stnerf_set_ray_ids": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64]),
     "stnerf_selftest_umma": (C.c_int, [C.POINTER(C.c_float)]),
-    "stnerf_selftest_umma_pair": (C.c_int, [C.POINTER(C.c_float)]),
-    "stnerf_selftest_umma_ts": (C.c_int, [C.POINTER(C.c_float)]),
     "stnerf_selftest_umma_accum": (C.c_int, [C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "stnerf_profile_begin": (C.c_int, [_P]),
     "stnerf_profile_end": (C.c_int, [_P, C.POINTER(Profile)]),
@@ -98,7 +96,7 @@ def lib():
     if _lib is None:
         if not os.path.isfile(LIB_PATH):
             raise StnerfError("%s not found -- build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                              "(the B200 path has no CPU fallback)" % LIB_PATH)
+                              "(the H100 path has no CPU fallback)" % LIB_PATH)
         L = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(L, name)

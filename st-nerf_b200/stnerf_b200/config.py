@@ -1,5 +1,5 @@
 """cfg stub for hosts without yacs: the fields `LayeredRFRender.__init__` reads (modeling/layered_rfrender.py:23-37),
-with the shipped configs' values (configs/config_taekwondo.yml:51-66), plus the two B200 knobs."""
+with the shipped configs' values (configs/config_taekwondo.yml:51-66), plus the two knobs of the native path."""
 import types
 
 

@@ -73,11 +73,11 @@ class LayeredRFRender(torch.nn.Module):
             raise NotImplementedError("SAMPLE_METHOD=%r: only 'BBOX' is usable in the reference (SURVEY A.9)" % M.SAMPLE_METHOD)
         for flag in ("POSE_REFINEMENT", "USE_DEFORM_VIEW", "BKGD_USE_DEFORM_TIME", "SAME_SPACENET"):
             if getattr(M, flag, False):
-                raise NotImplementedError("cfg.MODEL.%s=True is not part of the B200 hot path (disabled in every shipped config)" % flag)
+                raise NotImplementedError("cfg.MODEL.%s=True is not part of the native hot path (disabled in every shipped config)" % flag)
         if getattr(M, "DEEP_RGB", False) and M.USE_SPACE_TIME:
             raise NotImplementedError("DEEP_RGB head is not used by any shipped checkpoint")
         if not M.USE_DEFORM_TIME or not M.USE_DIR or not M.TKERNEL_INC_RAW:
-            raise NotImplementedError("the B200 path implements USE_DEFORM_TIME=USE_DIR=TKERNEL_INC_RAW=True (both shipped configs)")
+            raise NotImplementedError("the native path implements USE_DEFORM_TIME=USE_DIR=TKERNEL_INC_RAW=True (both shipped configs)")
         self.layer_num = int(cfg.DATASETS.LAYER_NUM)
         self.camera_num = camera_num
         self.coarse_ray_sample = int(M.COARSE_RAY_SAMPLING)
@@ -281,7 +281,7 @@ class LayeredRFRender(torch.nn.Module):
         else:
             raise ValueError("undefined ray format in LayeredRFRender, ray dimension is %d" % width)   # (:162-163)
         if not rays.is_cuda:
-            raise L.StnerfError("rays must be CUDA tensors: the B200 path has no CPU fallback")
+            raise L.StnerfError("rays must be CUDA tensors: the native path has no CPU fallback")
         if rays.size(0) < 2:
             raise ValueError("need more than one ray per call (layered_rfrender.py:309)")
         rays = rays.detach().to(torch.float32)

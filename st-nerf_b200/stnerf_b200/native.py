@@ -37,7 +37,7 @@ class NativeRenderer:
 
     def __init__(self, n_layers: int, space_time: Sequence[bool], precision: str = "fp32", chunk_rays: int = 0):
         if not torch.cuda.is_available():
-            raise L.StnerfError("stnerf_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise L.StnerfError("stnerf_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.l = int(n_layers)
         desc = L.ModelDesc()
         desc.n_layers = self.l

@@ -303,7 +303,7 @@ def write_synthetic_dataset(root: str, with_image: bool = True, spec: dict = Non
 # ---------------------------------------------------------------------------------------------------------------------
 # Parity at scale (BASELINE configs[1], configs[2] and the 64+192 sampling of configs[4]): thousands of rays of a full-size
 # view, spread evenly over the image.  `make_golden_scale.py` stores the UNMODIFIED reference's fine images for these inputs;
-# the gpu test compares the B200 path with them and attributes every pixel over the 1e-3 gate (tests/test_gpu_parity_scale.py).
+# the gpu test compares the native path with them and attributes every pixel over the 1e-3 gate (tests/test_gpu_parity_scale.py).
 # ---------------------------------------------------------------------------------------------------------------------
 SCALE_CASES = {
     "scale_tkd2_16k": dict(weights="taekwondo", L=2, space_time=True, n1=64, n2=128, frame_ids=[0, 10, 11], thr=(0.0, 0.0),

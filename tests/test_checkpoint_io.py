@@ -1,5 +1,7 @@
-"""Checkpoint discovery / loading and camera-file parsing (SURVEY 8f rows 3-4).  CPU only.  When the reference tree is
-present (build container) its own functions (data/datasets/utils.py, a numpy-only module) are executed side by side."""
+"""Checkpoint discovery / loading and camera-file parsing (SURVEY 8f rows 3-4).  CPU only.  The reference's own functions
+(data/datasets/utils.py, a numpy-only module) were run on the same inputs and their outputs stored in
+tests/golden/dataset_utils.npz (tests/golden/make_golden_dataset_utils.py); with $STNERF_REFERENCE_ROOT set they are also run
+side by side."""
 import importlib.util
 import os
 
@@ -10,13 +12,21 @@ import torch
 import cases as C
 from tests_support import make_cfg
 
-REF_UTILS = "/root/reference/data/datasets/utils.py"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "dataset_utils.npz")
+CKPT_NAMES = ("layered_rfnr_checkpoint_3.pt", "layered_rfnr_checkpoint_12.pt", "layered_rfnr_checkpoint_5_200.pt", "other.pt")
+
+
+def camera_inputs():
+    rs = np.random.RandomState(3)
+    return rs.rand(5, 9) * 1000, rs.rand(5, 12)
 
 
 def _ref():
-    if not os.path.isfile(REF_UTILS):
+    root = os.environ.get("STNERF_REFERENCE_ROOT")
+    path = os.path.join(root, "data", "datasets", "utils.py") if root else None
+    if not path or not os.path.isfile(path):
         return None
-    spec = importlib.util.spec_from_file_location("_ref_dataset_utils", REF_UTILS)
+    spec = importlib.util.spec_from_file_location("_ref_dataset_utils", path)
     m = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(m)
     return m
@@ -28,11 +38,14 @@ def test_get_iteration_path(tmp_path):
     d = str(tmp_path)
     assert io.get_iteration_path(os.path.join(d, "nope")) is None
     assert io.get_iteration_path(d) is None                                   # empty directory
-    for name in ("layered_rfnr_checkpoint_3.pt", "layered_rfnr_checkpoint_12.pt", "layered_rfnr_checkpoint_5_200.pt",
-                 "other.pt"):
+    gold = np.load(GOLDEN)
+    assert bool(gold["empty_dir_is_none"])
+    for name in CKPT_NAMES:
         open(os.path.join(d, name), "w").close()
     assert io.get_iteration_path(d) == os.path.join(d, "layered_rfnr_checkpoint_12.pt")
     assert io.get_iteration_path(d, fix_iter=7) == os.path.join(d, "frame", "layered_rfnr_checkpoint_7.pt")
+    assert os.path.relpath(io.get_iteration_path(d), d) == str(gold["latest"])               # what the reference returned
+    assert os.path.relpath(io.get_iteration_path(d, 7), d) == str(gold["fix_iter_7"])
     if ref is not None:
         assert io.get_iteration_path(d) == ref.get_iteration_path(d)
         assert io.get_iteration_path(d, 7) == ref.get_iteration_path(d, 7)
@@ -42,17 +55,18 @@ def test_get_iteration_path(tmp_path):
 def test_camera_file_parsing(tmp_path):
     from stnerf_b200 import checkpoint_io as io
     ref = _ref()
-    rs = np.random.RandomState(3)
-    Ks = rs.rand(5, 9) * 1000
+    Ks, poses = camera_inputs()
     fn = os.path.join(str(tmp_path), "K.txt")
     np.savetxt(fn, Ks)
     got = io.read_intrinsics(fn)
     assert got.shape == (5, 3, 3) and np.array_equal(got, np.loadtxt(fn).reshape(5, 3, 3))
-    poses = rs.rand(5, 12)
     ext = io.campose_to_extrinsic(poses)
     assert ext.shape == (5, 4, 4) and np.array_equal(ext[:, :3, :].reshape(5, 12), poses) and np.all(ext[:, 3] == [0, 0, 0, 1])
     with pytest.raises(Exception):
-        io.campose_to_extrinsic(rs.rand(5, 11))
+        io.campose_to_extrinsic(np.random.RandomState(4).rand(5, 11))
+    gold = np.load(GOLDEN)                                                         # what the reference returned
+    assert np.array_equal(got, gold["read_intrinsics"])
+    assert np.array_equal(ext, gold["campose_to_extrinsic"])
     if ref is not None:
         assert np.array_equal(got, ref.read_intrinsics(fn))
         assert np.array_equal(ext, ref.campose_to_extrinsic(poses))

@@ -3,7 +3,7 @@
 Executes the EXACT import block of the reference's demos (demo/taekwondo_demo.py:16-23, demo/walking_demo.py:16-24) in a
 fresh interpreter with that path order (cwd = reference root, `sys.path.append('.')` as the demos do, PYTHONPATH =
 st-nerf_b200) and third-party packages this image lacks (yacs, imageio, matplotlib, kornia) stubbed.  Hot-path names must
-come from the B200 facade, everything else (`engine.layered_trainer`, `config`, `solver`, `utils.metrics`) from the reference
+come from the native facade, everything else (`engine.layered_trainer`, `config`, `solver`, `utils.metrics`) from the reference
 through the facade packages' fall-through (`stnerf_b200/_fallthrough.py`).  A second test builds a miniature fake reference
 tree so the mechanism is covered where no reference checkout exists."""
 import os
@@ -37,7 +37,7 @@ CHECK = textwrap.dedent('''
     import engine, layers, utils, modeling, render, config, solver
     pkg = os.environ["STNERF_TEST_PKG"]; ref = os.path.realpath(os.getcwd())
     here = lambda m: os.path.realpath(sys.modules[m.__module__ if not hasattr(m, "__file__") else m.__name__].__file__)
-    # hot-path names: the B200 facade
+    # hot-path names: the native facade
     for obj in (make_loss, RaySamplePoint, batchify_ray, vis_density, LayeredNeuralRenderer, setup_logger):
         assert here(obj).startswith(pkg), (obj, here(obj))
     for mod in (engine, layers, utils, modeling, render):

@@ -78,7 +78,7 @@ def test_walking_demo_import_alias():
 
 
 def test_example_demo_runs(tmp_path):
-    """The scripted edit sessions of demo/taekwondo_demo.py on the B200 path (tiny size)."""
+    """The scripted edit sessions of demo/taekwondo_demo.py on the native path (tiny size)."""
     import os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, os.path.join(root, "examples", "taekwondo_demo_b200.py"), "--size", "96x54",

@@ -1,6 +1,6 @@
 """Randomised cross-check of the two MLP implementations on the GPU: for random layer counts / sample counts / ray counts
-the tcgen05 path (exact mode) must agree with the fp32 CUDA-core path on the same rays and the same in-kernel Philox
-uniforms, and must be bit-reproducible run to run.  A protocol bug in the warp-specialised kernel (barrier phase, TMEM
+the tensor-core path (exact mode) must agree with the fp32 CUDA-core path on the same rays and the same in-kernel Philox
+uniforms, and must be bit-reproducible run to run.  A protocol bug in the warp-specialised kernel (barrier phase, activation
 buffer reuse, ring slot reuse) shows up here as garbage or non-determinism."""
 import numpy as np
 import pytest

@@ -5,16 +5,15 @@ view (`tests/golden/make_golden_scale.py`).  The tensor-core modes `exact` and `
 gate (pixel RGB and opacity within 1e-3) on at least 99.8 % of the rays, with a median error below 5e-5 -- and EVERY ray over
 the gate must be attributed to an instability of the reference itself, or the test fails.
 
-Why a few rays exceed the gate (measured, `tests/tools/net_error_probe.py` -> profiles/): the tensor core adds into its fp32
-accumulator with truncation (about -1.7 * 2^-24 relative per K=16 MMA, `stnerf_selftest_umma_accum`), so the fp16x3 split
-reproduces sigma to 7e-6 rms relative where the reference's own fp32 GEMMs are 1e-6 from the float64 truth.  Two steps of the
-reference amplify such differences without bound:
+Why a few rays exceed the gate (`tests/tools/net_error_probe.py` measures it): the tensor core does not round its fp32
+accumulation like an fp32 FFMA chain (`stnerf_selftest_umma_accum`), so the fp16x3 split reproduces sigma slightly less
+closely than the reference's own fp32 GEMMs do.  Two steps of the reference amplify such differences without bound:
   * `utils/sample_pdf.py:58-61`: a fine depth is `bin_lo + (u - cdf_lo) / denom * width`; where the coarse pdf of a bin is tiny
     (empty space in front of / behind a surface: denom ~ 1e-5 .. 1e-3) a 1e-6 change of the cdf moves the sample by a visible
     fraction of the bin, and the fine network is steep there;
   * `modeling/layered_rfrender.py:416-418, 538-547, 564-566`: densities below a threshold are zeroed (walking: 20 / 0.8).
 Attribution, per ray over the gate (reference re-run out of process from the archive packed by oracle/stash_reference.py):
-  A  the reference, re-run with ITS fine depths replaced by the ones the B200 path chose, reproduces the B200 pixel (measured:
+  A  the reference, re-run with ITS fine depths replaced by the ones the native path chose, reproduces the native pixel (measured:
      to ~1e-6; asserted: a quarter of the gate) -- fine networks, thresholds and compositing agree exactly, the whole difference
      is where the fine samples were placed; and those placements are the reference's own up to its conditioning: every fine
      depth matches the reference's within the shift a cdf change of 1e-4 produces (`|dz| * denom / bin_width <= 1e-4`;
@@ -42,7 +41,7 @@ GATE = 1e-3
 MAX_OUTLIER_FRACTION = {False: 2e-3, True: 5e-3}     # without / with density thresholds (walking: 20 / 0.8 zero densities below them)
 UNSTABLE = GATE / 4
 PERTURB_REL = 1e-5
-SIGMA_REL = 3e-5                     # ~4 x the measured rms disagreement of the densities (profiles/r02_net_error_probe.json)
+SIGMA_REL = 3e-5                     # ~4 x the rms disagreement of the densities measured by tests/tools/net_error_probe.py
 SEEDS = (1, 2, 3, 4)
 MAX_ATTRIBUTED = 96                  # rays re-run through the reference per mode (all outliers in every shipped case)
 N_CONTROL = 48
@@ -133,7 +132,7 @@ def attribute_outliers(case, model, rays, jit, u, idx, flat_full, mixed=False):
         var = C.run_reference_job(C.reference_job(case, r_s, j_s, u_s, variants=variants))["variants"]
         _cache[key] = (base, var)
     ref, rec = base["flat"], base["record"]
-    on_b200_depths = _err(sub, var[0]["flat"], l)
+    on_native_depths = _err(sub, var[0]["flat"], l)
     score = np.max([_err(v["flat"], ref, l) for v in var[1:]], axis=0)       # how far the reference itself moves
     implied = np.zeros(n)
     for r in range(no):
@@ -144,22 +143,22 @@ def attribute_outliers(case, model, rays, jit, u, idx, flat_full, mixed=False):
     dump = os.path.join(C.ROOT, "gpurun_out")
     if os.path.isdir(dump):              # raw material for offline analysis (scratch, not asserted on)
         np.savez_compressed(os.path.join(dump, "attrib_%s_%s.npz" % (case["name"], model.precision)), sel=sel.numpy(), n_out=no, score=score,
-                            on_b200_depths=on_b200_depths, implied=implied, **{"tc%d" % i: tc[i] for i in range(l)},
+                            on_native_depths=on_native_depths, implied=implied, **{"tc%d" % i: tc[i] for i in range(l)},
                             **{"tf%d" % i: tf[i] for i in range(l)}, **{"sub." + k: v for k, v in sub.items()}, **{"ref." + k: v for k, v in ref.items()})
     labels, unattributed = [], []
     for r in range(no):
-        A = on_b200_depths[r] <= UNSTABLE and implied[r] <= CDF_EPS
+        A = on_native_depths[r] <= UNSTABLE and implied[r] <= CDF_EPS
         Cc = score[r] > UNSTABLE
         labels.append("placement" if A else ("unstable" if Cc else "unattributed"))
         if not (A or Cc):
-            unattributed.append((int(idx[r]), float(_err(sub, ref, l)[r]), float(on_b200_depths[r]), float(score[r])))
+            unattributed.append((int(idx[r]), float(_err(sub, ref, l)[r]), float(on_native_depths[r]), float(score[r])))
     if mixed:        # colour precision of the single-pass layer: small, rare, colour only (acc / depth untouched by construction)
         assert len(unattributed) <= 5e-4 * rays.shape[0] and all(e[1] <= 2.5e-3 for e in unattributed), unattributed
     else:
         assert not unattributed, "rays over the gate that are neither placement-explained nor unstable in the reference: %s" % unattributed
     assert (score[no:] < UNSTABLE).mean() >= 0.95, "ordinary rays are unstable too: %s" % np.sort(score[no:])[-5:]
     return {"rays_attributed": int(no), "labels": {k: labels.count(k) for k in sorted(set(labels))},
-            "max_err_of_reference_on_b200_depths_vs_b200": float(on_b200_depths[:no][[lb == "placement" for lb in labels]].max()) if "placement" in labels else None,
+            "max_err_of_reference_on_native_depths_vs_native": float(on_native_depths[:no][[lb == "placement" for lb in labels]].max()) if "placement" in labels else None,
             "max_implied_cdf_difference_of_placements": float(implied[:no].max()),
             "reference_move_under_perturbations": {"outliers_median": float(np.median(score[:no])), "controls_median": float(np.median(score[no:])),
                                                    "controls_p95": float(np.sort(score[no:])[int(0.95 * (n - no))])}}

@@ -1,7 +1,7 @@
 """GPU parity of the full hot path (through the facade -> C ABI) against the reference's golden outputs.
 
 Tolerance (BASELINE.json north_star): pixel RGB within 1e-3 of the reference on identical rays / weights / uniforms.
-fp32 and exact (3-term fp16 split on tcgen05) modes must meet it on every ray; depth is checked relatively
+fp32 and exact (3-term fp16 split on the tensor cores) modes must meet it on every ray; depth is checked relatively
 (depths reach ~10 and are sums of w*t)."""
 import numpy as np
 import pytest

@@ -147,31 +147,10 @@ def test_networks(tag, precision, sig_tol, rgb_tol):
 
 
 def test_umma_selftest():
-    """One 128x128x64 fp16 MMA through the library's UMMA descriptors / SW128 layout / bulk copy / TMEM load."""
+    """One 128x256x64 fp16 product through the library's warpgroup-MMA descriptors / swizzled layouts / bulk copy /
+    accumulator fragment."""
     import ctypes
     from stnerf_b200 import _lib as L
     err = ctypes.c_float(-1.0)
     L.check(L.lib().stnerf_selftest_umma(ctypes.byref(err)), "stnerf_selftest_umma")
     assert 0.0 <= err.value < 1e-3, err.value
-
-
-def test_umma_ts_selftest():
-    """The same product with the A operand in tensor memory, written with tcgen05.st in the SpaceNet epilogue's layout
-    (SPACE_A_TMEM: activations never leave tensor memory between layers)."""
-    import ctypes
-    from stnerf_b200 import _lib as L
-    err = ctypes.c_float(-1.0)
-    L.check(L.lib().stnerf_selftest_umma_ts(ctypes.byref(err)), "stnerf_selftest_umma_ts")
-    assert 0.0 <= err.value < 1e-3, err.value
-
-
-@pytest.mark.gpu
-def test_umma_pair_selftest():
-    """256x256x64 through ONE cta_group::2 accumulator: a 2-CTA cluster, each CTA holding its 128 rows of A and half of the B
-    rows, remote mbarrier arrives on the leader, multicast commit, paired TMEM allocation (the SPACE_CTA_PAIR protocol)."""
-    import ctypes
-    from stnerf_b200 import _lib as L
-    for _ in range(3):
-        err = ctypes.c_float(-1.0)
-        L.check(L.lib().stnerf_selftest_umma_pair(ctypes.byref(err)), "stnerf_selftest_umma_pair")
-        assert 0.0 <= err.value < 1e-3, err.value
