@@ -40,7 +40,7 @@ def main(out):
     pos = (torch.rand(n, 3, generator=g) * 4 - 2).cuda()
     dirs = torch.nn.functional.normalize(torch.randn(n, 3, generator=g), dim=1).cuda()
     tm = (torch.rand(n, generator=g) * 20).cuda()
-    for prec in ("exact", "exact_cf", "mixed"):
+    for prec in ("exact", "exact_cf", "mixed", "fast"):
         sd = O.synthetic_state_dict(1, True, seed=5)
         r = NativeRenderer(2, [False, True], prec)
         r.load_state_dict(sd)
@@ -51,16 +51,18 @@ def main(out):
         flow = r.motionnet(1, torch.cat([pos, tm[:, None]], 1))
         res["%s.flow" % prec] = flow.cpu().numpy()
         r.close()
-    # one small coarse + fine render (fused coarse compositing, flow reuse, fine pass)
-    for name in ("syn_L2_64_128", "tkd_edit_frac"):
+    # small coarse + fine renders (fused coarse compositing, flow reuse, fine pass); exact_cf adds the corrections first in
+    # the coarse pass and the MotionNets, interleaved in the fine pass
+    for name, prec in (("syn_L2_64_128", "exact"), ("tkd_edit_frac", "exact"), ("syn_L2_64_128", "exact_cf")):
         if name not in C.CASES:
             continue
-        flat = run_case_native(name, "exact")
+        flat = run_case_native(name, prec)
         if flat is None:
             continue
+        tag = name if prec == "exact" else "%s.%s" % (name, prec)
         for k, v in flat.items():
             v = np.asarray(v)
-            res["%s.%s" % (name, k)] = v.astype(np.float32) if v.dtype.kind == "f" else v
+            res["%s.%s" % (tag, k)] = v.astype(np.float32) if v.dtype.kind == "f" else v
     for k, v in res.items():
         if v.dtype.kind == "f" and not np.isfinite(v).all():
             print("WARNING: non-finite values in", k)

@@ -68,11 +68,6 @@ struct stnerf_ctx {
   std::vector<cudaEvent_t> ev_pool;                         // timing-disabled events, reused call after call
   float* box_table = nullptr;  // [n_frames][l][2][3] per-frame boxes for rays with their own frame id (stnerf_set_box_table)
   int box_frames = 0;
-  // Order of the split MMAs (mlp_tc.cu): 0 = interleaved everywhere, 1 = correction products first in the COARSE pass and in the
-  // MotionNets (what the sample placement and the positions depend on), interleaved in the fine SpaceNet pass, 2 = first everywhere.
-  // -1 (default): by precision -- STNERF_PREC_TC_3XF16_CF means 1, every other mode 0.
-  int lo_first_env = -1;       // STNERF_LO_FIRST=0|1|2 in the environment at create overrides (A/B experiments)
-  int lo_first_mode() const { return lo_first_env >= 0 ? lo_first_env : (precision == STNERF_PREC_TC_3XF16_CF ? 1 : 0); }
   bool no_fuse = false;        // STNERF_NO_FUSE=1 in the environment at create: keep the coarse compositing in its own kernel (A/B)
   int* any_frac = nullptr;     // scratch flag for stnerf_motionnet(lerp_mode=-1)
   RayIdMap idmap{0, 0, 0};     // stnerf_set_ray_ids
@@ -195,7 +190,6 @@ int stnerf_create(stnerf_handle* out, const stnerf_model_desc* d) {
   c->precision = d->precision;
   c->chunk_rays = d->chunk_rays > 0 ? d->chunk_rays : 65536;
   if (const char* e = getenv("STNERF_NO_FUSE")) c->no_fuse = (e[0] == '1');
-  if (const char* e = getenv("STNERF_LO_FIRST")) c->lo_first_env = (e[0] == '1') ? 1 : (e[0] == '2') ? 2 : 0;
   if (const char* e = getenv("STNERF_NO_REUSE")) c->no_reuse = (e[0] == '1');
   if (cudaMalloc((void**)&c->any_frac, 4) != cudaSuccess) { delete c; return STNERF_ENOMEM; }
   *out = c;
@@ -317,7 +311,7 @@ int stnerf_load_motionnet(stnerf_handle c, int layer, const float* blob, size_t 
 // ---- packed-weight image (SURVEY 8f row 3): every loaded network's device buffers, as they are, behind a small header ----
 namespace {
 constexpr char PACK_MAGIC[8] = {'S', 'T', 'N', 'B', '2', '0', '0', 'W'};
-constexpr uint32_t PACK_VERSION = 3;      // 2: weight stream = correction section + main section per layer; 3: skip layer's encoding chunk first
+constexpr uint32_t PACK_VERSION = 4;      // 4: weight stream = (hi, lo) stage per 32-k sub-chunk, each stage stored once
 struct PackHeader { char magic[8]; uint32_t version, n_layers, n_records, reserved; };
 struct PackRec { uint32_t kind, fine, layer, use_time; uint64_t simt_floats, stream_bytes, aux_floats, tail_floats; float scalars[4]; uint32_t pad[4]; };
 static size_t rec_payload(const PackRec& r) { return r.simt_floats * 4 + r.stream_bytes + r.aux_floats * 4 + r.tail_floats * 4; }
@@ -477,12 +471,11 @@ static int run_spacenet(stnerf_ctx* c, const PointSrc& src, SpaceNetDev& net, fl
   if (src.mode == SRC_EXPLICIT) {      // unit entry point: one bias row per point, stream-ordered scratch
     float* cb = nullptr;
     STNERF_CUDA(cudaMallocAsync((void**)&cb, (size_t)std::max<long long>(src.n_slots, 1) * 128 * sizeof(float), st));
-    const int rc = tc_launch_spacenet(src, net.tc, net.w, c->precision, cb, raw, rgb, sigma, c->num_sms, st, nullptr, c->lo_first_mode() != 0);
+    const int rc = tc_launch_spacenet(src, net.tc, c->precision, cb, raw, rgb, sigma, c->num_sms, st);
     STNERF_CUDA(cudaFreeAsync(cb, st));
     return rc;
   }
-  const int lo_first = c->lo_first_mode() == 2 || (c->lo_first_mode() == 1 && !fine_pass);
-  return tc_launch_spacenet(src, net.tc, net.w, c->precision, c->cbuf, raw, rgb, sigma, c->num_sms, st, fuse, lo_first);
+  return tc_launch_spacenet(src, net.tc, c->precision, c->cbuf, raw, rgb, sigma, c->num_sms, st, fuse, fine_pass);
 }
 static int run_motionnet(stnerf_ctx* c, const PointSrc& src, MotionNetDev& net, const int* lerp_flag, int lerp_force,
                          float* xyz_out, float* flow_out, cudaStream_t st, int count_slot = -1) {
@@ -490,8 +483,7 @@ static int run_motionnet(stnerf_ctx* c, const PointSrc& src, MotionNetDev& net, 
   ProfScope ps(c, 1, (double)src.n_slots * src.S, count_slot, src.S, st);
   if (c->precision == STNERF_PREC_FP32_SIMT)
     return launch_motionnet_simt(src, net.w, lerp_flag, lerp_force, xyz_out, flow_out, c->num_sms, st);
-  return tc_launch_motionnet(src, net.tc, net.w, c->precision, lerp_flag, lerp_force, xyz_out, flow_out, c->num_sms, st,
-                             c->lo_first_mode() != 0);
+  return tc_launch_motionnet(src, net.tc, c->precision, lerp_flag, lerp_force, xyz_out, flow_out, c->num_sms, st);
 }
 
 // `fuse` (coarse pass only): template of the per-layer fusion request (everything but the layer-specific fields), or null.

@@ -9,16 +9,17 @@
 //   * activations (A operand) live in shared memory as fp16 hi/lo pairs in the canonical 128B-swizzled K-major layout
 //     ([128 rows x 64 k] blocks); a layer's epilogue overwrites the rows its own MMAs have just finished reading;
 //   * weights (B operand) are pre-packed on the host into [N out-rows x 32 k] fp16 blocks that are already the 64B-swizzled
-//     shared-memory image, in the exact order the math warpgroups consume them, and stream through a ring of stages with 1-D
-//     bulk async copies (cp.async.bulk + mbarrier complete_tx) from L2; a slot is refilled once every math warp has seen the
-//     MMAs that read it retire (wgmma.wait_group);
+//     shared-memory image -- per layer the hi and then the lo stage of every 32-k sub-chunk, in the layer's K order, each
+//     stored once -- and stream through a ring of stages with 1-D bulk async copies (cp.async.bulk + mbarrier complete_tx) from
+//     L2, in the order of the layer's steps (WSched); a slot is refilled once every math warp has seen the MMAs that read it
+//     retire (wgmma.wait_group);
 //   * exact mode issues three fp16 MMAs per product, D += Ahi*Whi + Alo*Whi + Ahi*Wlo (fp32 accumulate), which reproduces fp32
 //     products to ~2^-22 (SURVEY App. C.3: the only tensor-core formulation inside the 1e-3 gate); mixed mode keeps that
 //     everywhere the density depends on and runs the colour-only layer rgb_net.1 in one pass;
 //   * order of the three products (template parameter LOFIRST): interleaved per 32-k sub-chunk (default: every weight stage is
 //     streamed once), or -- TC_3XF16_CF "exact_cf", coarse pass + MotionNets -- the two correction products FIRST over the whole K
 //     range, then Ahi*Whi, so the accumulator is small while the corrections are added (stnerf_selftest_umma_accum measures how
-//     the tensor core rounds its fp32 accumulation); the hi weight stages are then streamed twice;
+//     the tensor core rounds its fp32 accumulation); the hi weight stages are then streamed twice (stored once);
 //   * relu(PE(dir) | PE(time)) enters rgb_net.1 as a per-ray fp32 bias computed by head_bias_kernel
 //     (b1 + W1[:,256:] . relu(enc)), so the last GEMM is a clean K=256;
 //   * the 1-wide density head, the 3-wide rgb / flow heads and all biases are fp32 FFMA work in the epilogue;
@@ -241,25 +242,89 @@ template <> struct Sched<NET_MOTION> {
 };
 static_assert(Sched<NET_SPACE>::n_stage <= MAX_STAGE && Sched<NET_MOTION>::n_stage <= MAX_STAGE, "barrier slots");
 
+// Weight schedule of a layer: the one definition of the order in which the producer streams the weight stages and the math
+// warpgroups consume them.  A layer's section of the stream holds, per 32-k sub-chunk in the layer's K order, the hi stage and
+// then the lo stage ([n_out rows x 32 k] fp16 each).  Each step loads one stage and multiplies it with the A slice of one
+// sub-chunk:
+//   * interleaved split (exact, mixed): per sub-chunk the lo stage (Ahi*Wlo), then the hi stage (Ahi*Whi, then Alo*Whi);
+//   * corrections first (LOFIRST, exact_cf): per sub-chunk the lo stage (Ahi*Wlo) and the hi stage (Alo*Whi) over the whole
+//     K range, then every hi stage again (Ahi*Whi);
+//   * single pass (fast, and the last layer in mixed): the hi stages only (Ahi*Whi).
+enum { A_HI = 0, A_LO = 1, A_HI_LO = 2 };     // A operand of a step: Ahi, Alo, or Ahi then Alo (two MMA pairs off one stage)
+template <int A>
+struct WStep {
+  static constexpr int a = A;
+  uint32_t offset;                            // byte offset of the step's weight stage inside the layer's section
+  uint32_t sub;                               // 32-k sub-chunk of the A chunk
+};
+template <int NET>
+struct WSched {
+  using S = Sched<NET>;
+  __host__ __device__ static constexpr int n_chunks(int l) { return S::act_chunks(l) + S::enc_chunks(l); }
+  __host__ __device__ static constexpr uint32_t stage_bytes(int l) { return (uint32_t)S::n_out(l) * 64; }
+  __host__ __device__ static constexpr size_t layer_bytes(int l) { return (size_t)n_chunks(l) * 2 /*sub-chunks*/ * 2 /*hi, lo*/ * stage_bytes(l); }
+  // chunk id (activation chunks 0 .. act_chunks-1, then the encoding chunks) at position c of the layer's K order: the skip
+  // layer takes its encoding chunk first
+  __host__ __device__ static constexpr int chunk_at(int l, int c) {
+    return S::enc_first(l) ? (c == 0 ? S::act_chunks(l) : c - 1) : c;
+  }
+  static constexpr bool enc_first_valid() {
+    for (int l = 0; l < S::N_LAYERS; ++l)
+      if (S::enc_first(l) && (S::act_chunks(l) == 0 || S::enc_chunks(l) == 0)) return false;
+    return true;
+  }
+  static_assert(enc_first_valid(), "enc_first(l) needs activation chunks and an encoding chunk to reorder");
+  // The steps of layer l, in order: per A chunk, a = chunk(chunk id) once, then f(a, WStep<A>) for every step on that chunk.
+  // The operand is a compile-time constant, so every kind of step is a separate, straight-line copy of f.
+  template <bool LOFIRST, class C, class F>
+  __device__ __forceinline__ static void for_each_step(int l, bool split, C&& chunk, F&& f) {
+    // written out rather than n_chunks(l): with the call, nvcc fully unrolls the MotionNet correction pass, and that kernel spills
+    const int nact = S::act_chunks(l), nch = nact + S::enc_chunks(l);
+    const uint32_t bytes = stage_bytes(l);
+    auto at = [&](const auto& a, int c, uint32_t sub, uint32_t lo_stage, auto op) {
+      f(a, WStep<decltype(op)::value>{(2 * (2 * (uint32_t)c + sub) + lo_stage) * bytes, sub});
+    };
+    using HI = std::integral_constant<int, A_HI>;
+    using LO = std::integral_constant<int, A_LO>;
+    using HI_LO = std::integral_constant<int, A_HI_LO>;
+    if (!LOFIRST || !split) {
+      for (int c = 0; c < nch; ++c) {
+        const auto a = chunk(chunk_at(l, c));
+        for (uint32_t sub = 0; sub < 2; ++sub) {
+          if (split) { at(a, c, sub, 1u, HI()); at(a, c, sub, 0u, HI_LO()); }
+          else at(a, c, sub, 0u, HI());
+        }
+      }
+    } else {
+      for (int c = 0; c < nch; ++c) {
+        const auto a = chunk(chunk_at(l, c));
+        for (uint32_t sub = 0; sub < 2; ++sub) { at(a, c, sub, 1u, HI()); at(a, c, sub, 0u, LO()); }
+      }
+      for (int c = 0; c < nch; ++c) {
+        const auto a = chunk(chunk_at(l, c));
+        for (uint32_t sub = 0; sub < 2; ++sub) at(a, c, sub, 0u, HI());
+      }
+    }
+  }
+};
+
 template <int NET>
 __host__ __device__ constexpr size_t stream_bytes_per_tile() {
   size_t n = 0;
-  for (int l = 0; l < Sched<NET>::N_LAYERS; ++l)
-    n += (size_t)(Sched<NET>::act_chunks(l) + Sched<NET>::enc_chunks(l)) * 2 /*sub-chunks*/ * 3 /*correction pass: hi, lo; main pass: hi*/ *
-         Sched<NET>::n_out(l) * 64;
+  for (int l = 0; l < Sched<NET>::N_LAYERS; ++l) n += WSched<NET>::layer_bytes(l);
   return n;
 }
 
 struct TcParams {
   FuseCoarse fuse;            // SpaceNet, coarse pass: per-layer compositing + resampling in the compositing warps
   PointSrc src;
-  const uint8_t* wstream;     // packed weight stream (hi/lo stages in consumption order)
+  const uint8_t* wstream;     // packed weight stream (per layer: hi, lo stage per 32-k sub-chunk; see WSched)
   const float* aux;           // fp32: biases [8][256] | w_sigma[256] | b_sigma | w_out[3][128] | b_out[3]
   const float* cbuf;          // SpaceNet: per-slot rgb_net.1 bias (b1 + W1[:,256:].relu(enc(dir,time))), [slots][128]
   int exact;                  // 1: 3-term split, 0: single fp16 pass
   int single_last;            // with exact: the LAST GEMM layer (SpaceNet rgb_net.1, colour branch only) runs a single pass
   int lo_first;               // split layers (selects the kernel instantiation): 0 = interleaved per 32-k sub-chunk (hi stages
-                              // streamed once); 1 = correction products first over the whole K range, then Ahi*Whi
+                              // streamed once); 1 = correction products first over the whole K range, then Ahi*Whi (WSched)
   // outputs
   float* raw;                 // float4 per sample (pipeline mode)
   float* rgb_out;             // explicit mode
@@ -457,14 +522,13 @@ __device__ __forceinline__ void encode_piece(uint8_t* smem, const Pt& pt, int ro
 // warp `j` composites slot 2*tile+j from the rows the epilogue warps left in `rows` (float4 per row: rgb logits, sigma).
 template <int NZ>
 __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float* rows, float* cdf, uint32_t bar_full, uint32_t bar_empty,
-                                                  long long n_tiles, int j, int lane, bool clustered) {
+                                                  long long n_tiles, int j, int lane) {
   const FuseCoarse& F = P.fuse;
   const PointSrc& src = P.src;
   const long long n_slots = src.count ? (long long)(*src.count) : src.n_slots;
   const int n1 = 64, n2 = F.n2;
   uint32_t n = 0;
-  // (clustered: the CTAs of a cluster run the same number of tiles, the odd one out a tile past the end -- all slots invalid)
-  for (long long tile = blockIdx.x; clustered ? ((tile & ~1LL) < n_tiles) : (tile < n_tiles); tile += gridDim.x, ++n) {
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++n) {
     mbar_wait(bar_full, n & 1);
     const long long slot = tile * 2 + j;
     if (slot < n_slots) {
@@ -517,43 +581,28 @@ __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float
 // ---------------------------------------------------------------------------------------------------------
 // the kernel: one layer of a math warpgroup
 // ---------------------------------------------------------------------------------------------------------
-// MMAs of layer l for this warpgroup's 64 rows (A rows at byte offset a_row of every activation / encoding block), consuming the
-// weight stages in the order the producer streams them.  A stage is handed back (one arrival per math warp on w_empty) once the
-// MMAs that read it have retired: wgmma.wait_group 1 after the next stage's MMAs are issued keeps one stage of MMAs in flight.
+// MMAs of layer l for this warpgroup's 64 rows (A rows at byte offset a_row of every activation / encoding block), one weight
+// stage per step of WSched.  A stage is handed back (one arrival per math warp on w_empty) once the MMAs that read it have
+// retired: wgmma.wait_group 1 after the next stage's MMAs are issued keeps one stage of MMAs in flight.
 template <int NET, int N, bool LOFIRST>
 __device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uint32_t sbase, uint32_t a_row, uint32_t bars,
                                           uint32_t& cnt, int lane) {
   using S = Sched<NET>;
+  using W = WSched<NET>;
   constexpr uint32_t NST = S::n_stage;
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
   acc_fence<N / 2>(acc);
   wgmma_fence();
-  const int nact = S::act_chunks(l), nch = nact + S::enc_chunks(l);
+  const int nact = S::act_chunks(l);
   int pend = -1;
   auto release = [&](int s) {
     __syncwarp();
     mbar_arrive_if(bars + 8u * (uint32_t)(BAR_WEMPTY + s), lane == 0);
   };
-  // the next weight stage of the stream times the 32-k slice at a0 (and, two == true, at a1 as well)
-  auto stage = [&](uint32_t a0, uint32_t a1, auto two) {
-    const uint32_t s = cnt % NST, n = cnt / NST;
-    mbar_wait(bars + 8u * (BAR_WFULL + s), n & 1);
-    const uint32_t w = sbase + S::ring_base + s * S::stage_bytes;
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a0 + ks * 32), desc_sw64(w + ks * 32));
-    if (decltype(two)::value) {
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a1 + ks * 32), desc_sw64(w + ks * 32));
-    }
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (pend >= 0) release(pend);
-    pend = (int)s;
-    ++cnt;
-  };
   // hi / lo halves of A chunk ch (64 k): activation chunks 0..nact-1, then the encoding chunks
-  auto a_block = [&](int ch, uint32_t& hi, uint32_t& lo) {
+  auto a_block = [&](int ch) {
+    uint32_t hi, lo;
     if (ch < nact) {
       hi = sbase + S::act_base + ch * ABLOCK + a_row;
       lo = hi + S::LO_STRIDE;
@@ -561,39 +610,26 @@ __device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uin
       hi = sbase + S::enc_base + (ch - nact) * ABLOCK + a_row;
       lo = hi + S::ENC_LO_STRIDE;
     }
+    return make_uint2(hi, lo);
   };
-  // position c of the layer's K order -> chunk id
-  auto chunk_at = [&](int c) { return (S::enc_first(l) && nact > 0 && nch > nact) ? (c == 0 ? nact : c - 1) : c; };
-  if (!LOFIRST || !sp) {
-    // interleaved order (and single-pass layers): per 32-k sub-chunk Ahi*Wlo off the lo stage, then Ahi*Whi and Alo*Whi off the hi stage
-    for (int c = 0; c < nch; ++c) {
-      uint32_t hi, lo;
-      a_block(chunk_at(c), hi, lo);
-      for (uint32_t sub = 0; sub < 2; ++sub) {
-        if (sp) {
-          stage(hi + 64u * sub, 0u, std::false_type());
-          stage(hi + 64u * sub, lo + 64u * sub, std::true_type());
-        } else {
-          stage(hi + 64u * sub, 0u, std::false_type());
-        }
-      }
+  W::template for_each_step<LOFIRST>(l, sp, a_block, [&](const uint2& a, auto st) {
+    const uint32_t hi = a.x + 64u * st.sub, lo = a.y + 64u * st.sub;
+    const uint32_t a0 = decltype(st)::a == A_LO ? lo : hi;
+    const uint32_t s = cnt % NST, n = cnt / NST;
+    mbar_wait(bars + 8u * (BAR_WFULL + s), n & 1);
+    const uint32_t w = sbase + S::ring_base + s * S::stage_bytes;
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a0 + ks * 32), desc_sw64(w + ks * 32));
+    if constexpr (decltype(st)::a == A_HI_LO) {
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(lo + ks * 32), desc_sw64(w + ks * 32));
     }
-  } else {
-    // corrections first: D = Ahi*Wlo + Alo*Whi over the whole K range, then D += Ahi*Whi off the main section
-    for (int c = 0; c < nch; ++c) {
-      uint32_t hi, lo;
-      a_block(chunk_at(c), hi, lo);
-      for (uint32_t sub = 0; sub < 2; ++sub) {
-        stage(hi + 64u * sub, 0u, std::false_type());          // lo weight stage
-        stage(lo + 64u * sub, 0u, std::false_type());          // hi weight stage
-      }
-    }
-    for (int c = 0; c < nch; ++c) {
-      uint32_t hi, lo;
-      a_block(chunk_at(c), hi, lo);
-      for (uint32_t sub = 0; sub < 2; ++sub) stage(hi + 64u * sub, 0u, std::false_type());
-    }
-  }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (pend >= 0) release(pend);
+    pend = (int)s;
+    ++cnt;
+  });
   wgmma_wait<0>();
   acc_fence<N / 2>(acc);
   release(pend);
@@ -673,34 +709,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_consta
 
   if (warp == 0) {
     // =============================== weight producer: the whole warp runs the loop, one elected lane issues ===============================
+    using W = WSched<NET>;
     uint32_t cnt = 0;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const uint8_t* src = P.wstream;
+      const uint8_t* layer = P.wstream;
       for (int l = 0; l < S::N_LAYERS; ++l) {
-        const int nsub = 2 * (S::act_chunks(l) + S::enc_chunks(l));
-        const uint32_t bytes = (uint32_t)S::n_out(l) * 64;
-        const bool sp = split(l);
-        auto LOAD = [&](const uint8_t* stage) {
+        W::template for_each_step<LOFIRST>(l, split(l), [](int) { return 0; }, [&](int, auto st) {
           const uint32_t s = cnt % NST, n = cnt / NST;
           mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
-          load_stage_elect(sbase + S::ring_base + s * S::stage_bytes, stage, bytes, BAR(BAR_WFULL + s));
+          load_stage_elect(sbase + S::ring_base + s * S::stage_bytes, layer + st.offset, W::stage_bytes(l), BAR(BAR_WFULL + s));
           ++cnt;
-        };
-        // a layer of the stream = correction section [(hi, lo) per 32-k sub-chunk] + main section [hi per sub-chunk]
-        const uint8_t* corr = src;
-        const uint8_t* mainp = src + (size_t)nsub * 2 * bytes;
-        // the lo stage is consumed first (Ahi*Wlo), so it is loaded first
-        if (!LOFIRST) {       // interleaved order: the (lo, hi) stages of the correction section serve all three products;
-          for (int sc = 0; sc < nsub; ++sc) {                      // single-pass layers never touch the lo stages
-            if (sp) LOAD(corr + (size_t)(2 * sc + 1) * bytes);
-            LOAD(corr + (size_t)(2 * sc) * bytes);
-          }
-        } else {
-          if (sp)
-            for (int sc = 0; sc < nsub; ++sc) { LOAD(corr + (size_t)(2 * sc + 1) * bytes); LOAD(corr + (size_t)(2 * sc) * bytes); }
-          for (int sc = 0; sc < nsub; ++sc) LOAD(mainp + (size_t)sc * bytes);
-        }
-        src = mainp + (size_t)nsub * bytes;
+        });
+        layer += W::layer_bytes(l);
       }
     }
   } else if (NET == NET_SPACE && (warp == 2 || warp == 3)) {
@@ -709,9 +729,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_consta
       const int j = warp - 2;
       float* cdf = reinterpret_cast<float*>(smem + S::misc_base + MISC_CDF) + j * 64;
       if (P.fuse.n2 <= 128)
-        fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane, false);
+        fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
       else
-        fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane, false);
+        fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
     }
   } else if (wgi >= MATH_WG0) {
     // =============================== math warpgroups: encoding, MMAs, epilogues ===============================
@@ -947,7 +967,8 @@ __global__ void __launch_bounds__(256, 1) wgmma_selftest_kernel(const float* __r
 // host: weight packing
 // ---------------------------------------------------------------------------------------------------------
 // One layer of the stream.  W is (N, K_total) row-major.  A 64-wide k-chunk is described by the 64 source columns it
-// multiplies (-1 = zero padding), in the column order the device writes its A operand.
+// multiplies (-1 = zero padding), in the column order the device writes its A operand; `chunks` is indexed by chunk id
+// (activation chunks, then encoding chunks), the stream takes them in WSched::chunk_at order.
 struct LayerSpec { const float* W; int N, K_total; std::vector<std::vector<int>> chunks; };
 
 std::vector<int> iota_chunk(int k0, int kend) {
@@ -975,12 +996,14 @@ std::vector<std::vector<int>> enc_perm_motion() {
   return out;
 }
 
-int pack_stream(TcNet& net, const std::vector<LayerSpec>& layers, const std::vector<float>& aux, size_t expect_bytes) {
+template <int NET>
+int pack_stream(TcNet& net, const std::vector<LayerSpec>& layers, const std::vector<float>& aux) {
   std::vector<uint8_t> stream;
-  for (const LayerSpec& L : layers) {
+  for (int l = 0; l < (int)layers.size(); ++l) {
+    const LayerSpec& L = layers[l];
     const size_t stage = (size_t)L.N * 64;
-    std::vector<uint8_t> main_section;            // the hi stages again, consumed by the main pass (Ahi*Whi) after the correction pass
-    for (const auto& ch : L.chunks)
+    for (int c = 0; c < (int)L.chunks.size(); ++c) {
+      const std::vector<int>& ch = L.chunks[WSched<NET>::chunk_at(l, c)];
       for (int sub = 0; sub < 2; ++sub) {
         std::vector<uint8_t> hi(stage, 0), lo(stage, 0);
         for (int n = 0; n < L.N; ++n)
@@ -994,13 +1017,12 @@ int pack_stream(TcNet& net, const std::vector<LayerSpec>& layers, const std::vec
             memcpy(hi.data() + off, &h, 2);
             memcpy(lo.data() + off, &l, 2);
           }
-        stream.insert(stream.end(), hi.begin(), hi.end());          // correction section: (hi, lo) per 32-k sub-chunk
+        stream.insert(stream.end(), hi.begin(), hi.end());
         stream.insert(stream.end(), lo.begin(), lo.end());
-        main_section.insert(main_section.end(), hi.begin(), hi.end());
       }
-    stream.insert(stream.end(), main_section.begin(), main_section.end());
+    }
   }
-  if (stream.size() != expect_bytes) return STNERF_EINVAL;
+  if (stream.size() != stream_bytes_per_tile<NET>()) return STNERF_EINVAL;
   tc_free(net);
   net.blob_bytes = stream.size();
   STNERF_CUDA(cudaMalloc(&net.blob, stream.size()));
@@ -1054,11 +1076,8 @@ int tc_pack_spacenet(TcNet& net, const float* p, bool use_time) {
   for (int i = 0; i < 7; ++i) {
     LayerSpec L;
     L.W = p; L.N = HID; L.K_total = Ks[i];
-    const bool enc_first = Sched<NET_SPACE>::enc_first(i);
-    if (i == 4 && enc_first) L.chunks.push_back(enc_perm_space(HID));   // cat[x, PE(pos)] (spacenet.py:137): consumed first
     if (i != 0) for (int k = 0; k < HID; k += 64) L.chunks.push_back(iota_chunk(k, HID));
-    if (i == 0) L.chunks.push_back(enc_perm_space(0));
-    if (i == 4 && !enc_first) L.chunks.push_back(enc_perm_space(HID));
+    if (i == 0 || i == 4) L.chunks.push_back(enc_perm_space(i == 0 ? 0 : HID));   // layer 4: cat[x, PE(pos)] (spacenet.py:137)
     layers.push_back(L);
     p += (size_t)HID * Ks[i];
     memcpy(aux.data() + AUX_BIAS + i * 256, p, HID * sizeof(float));
@@ -1079,7 +1098,7 @@ int tc_pack_spacenet(TcNet& net, const float* p, bool use_time) {
   memcpy(aux.data() + AUX_WOUT, p, 3 * HEAD * sizeof(float)); p += 3 * HEAD;
   memcpy(aux.data() + AUX_BOUT, p, 3 * sizeof(float));
   net.use_time = use_time ? 1 : 0;
-  const int rc = pack_stream(net, layers, aux, stream_bytes_per_tile<NET_SPACE>());
+  const int rc = pack_stream<NET_SPACE>(net, layers, aux);
   if (rc) return rc;
   STNERF_CUDA(cudaMalloc((void**)&net.w_tail, tail.size() * sizeof(float)));
   STNERF_CUDA(cudaMemcpy(net.w_tail, tail.data(), tail.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -1102,7 +1121,7 @@ int tc_pack_motionnet(TcNet& net, const float* p) {
   }
   memcpy(aux.data() + AUX_WOUT, p, 3 * HEAD * sizeof(float)); p += 3 * HEAD;
   memcpy(aux.data() + AUX_BOUT, p, 3 * sizeof(float));
-  return pack_stream(net, layers, aux, stream_bytes_per_tile<NET_MOTION>());
+  return pack_stream<NET_MOTION>(net, layers, aux);
 }
 
 
@@ -1173,8 +1192,8 @@ static int launch_tc(const TcParams& P, int num_sms, cudaStream_t st) {
 
 bool tc_can_fuse_coarse(int n1, int n2) { return n1 == 64 && n2 >= 1 && n2 <= 256; }
 
-int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW&, int precision, float* cbuf, float* raw,
-                       float* rgb_out, float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse, int lo_first) {
+int tc_launch_spacenet(const PointSrc& src, const TcNet& net, int precision, float* cbuf, float* raw,
+                       float* rgb_out, float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse, bool fine_pass) {
   if (!net.blob || !net.w_tail) return STNERF_ENOWEIGHTS;
   if (!cbuf) return STNERF_EINVAL;
   // per-slot bias of rgb_net.1 (dir/time part), then the fused MLP
@@ -1192,7 +1211,9 @@ int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW&, 
   P.exact = precision == STNERF_PREC_TC_3XF16 || precision == STNERF_PREC_TC_MIXED || precision == STNERF_PREC_TC_3XF16_CF;
   P.single_last = precision == STNERF_PREC_TC_MIXED;
   P.raw = raw; P.rgb_out = rgb_out; P.sigma_out = sigma_out; P.lerp_force = 0;
-  P.lo_first = lo_first;
+  // exact_cf adds the corrections first where the sample placement and the positions depend on the result: the coarse pass and
+  // the MotionNets (and the unit entry points).  The fine SpaceNet pass keeps the interleaved order, which streams every stage once.
+  P.lo_first = precision == STNERF_PREC_TC_3XF16_CF && !fine_pass;
   if (fuse && fuse->on) {
     if (src.mode == SRC_EXPLICIT || src.S != 64 || !tc_can_fuse_coarse(fuse->n1, fuse->n2) || !fuse->t_fine) return STNERF_EINVAL;
     P.fuse = *fuse;
@@ -1200,15 +1221,15 @@ int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW&, 
   return launch_tc<NET_SPACE>(P, num_sms, st);
 }
 
-int tc_launch_motionnet(const PointSrc& src, const TcNet& net, const MotionNetW&, int precision, const int* lerp_flag_dev,
-                        int lerp_force, float* xyz_out, float* flow_out, int num_sms, cudaStream_t st, int lo_first) {
+int tc_launch_motionnet(const PointSrc& src, const TcNet& net, int precision, const int* lerp_flag_dev,
+                        int lerp_force, float* xyz_out, float* flow_out, int num_sms, cudaStream_t st) {
   if (!net.blob) return STNERF_ENOWEIGHTS;
   TcParams P;
   memset(&P, 0, sizeof(P));
   P.src = src; P.wstream = (const uint8_t*)net.blob; P.aux = net.aux;
   P.exact = precision == STNERF_PREC_TC_3XF16 || precision == STNERF_PREC_TC_MIXED || precision == STNERF_PREC_TC_3XF16_CF;      // the flow feeds positions: always split
   P.xyz_out = xyz_out; P.flow_out = flow_out; P.lerp_flag = lerp_flag_dev; P.lerp_force = lerp_force;
-  P.lo_first = lo_first;
+  P.lo_first = precision == STNERF_PREC_TC_3XF16_CF;
   return launch_tc<NET_MOTION>(P, num_sms, st);
 }
 

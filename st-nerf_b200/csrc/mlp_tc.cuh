@@ -46,12 +46,11 @@ int tc_export(const TcNet& net, bool is_space, uint8_t* stream_host, float* aux_
 int tc_import(TcNet& net, bool is_space, int use_time, const uint8_t* stream_host, const float* aux_host, const float* tail_host);
 int tc_selftest(float* max_err_host);   // one 128x256x64 warpgroup-MMA product vs a host reference
 int tc_selftest_accum(int reps, float* max_err_host, float* mean_signed_rel_host);   // accumulation probe (see mlp_tc.cu)
-int tc_launch_spacenet(const PointSrc& src, const TcNet& net, const SpaceNetW& w32, int precision, float* cbuf, float* raw,
-                       float* rgb_out, float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse = nullptr,
-                       int lo_first = 0);
+// fine_pass: the SpaceNet evaluation of a render's fine pass, which keeps the interleaved product order in TC_3XF16_CF
+int tc_launch_spacenet(const PointSrc& src, const TcNet& net, int precision, float* cbuf, float* raw, float* rgb_out,
+                       float* sigma_out, int num_sms, cudaStream_t st, const FuseCoarse* fuse = nullptr, bool fine_pass = false);
 bool tc_can_fuse_coarse(int n1, int n2);     // sample counts the fused compositing warps are instantiated for
-int tc_launch_motionnet(const PointSrc& src, const TcNet& net, const MotionNetW& w32, int precision,
-                        const int* lerp_flag_dev, int lerp_force, float* xyz_out, float* flow_out, int num_sms,
-                        cudaStream_t st, int lo_first = 0);
+int tc_launch_motionnet(const PointSrc& src, const TcNet& net, int precision, const int* lerp_flag_dev, int lerp_force,
+                        float* xyz_out, float* flow_out, int num_sms, cudaStream_t st);
 
 }  // namespace stnerf

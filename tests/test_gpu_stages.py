@@ -125,7 +125,7 @@ def _renderer(tag, precision):
     return r
 
 
-@pytest.mark.parametrize("precision,sig_tol,rgb_tol", [("fp32", 2e-3, 2e-4), ("exact", 2e-2, 2e-3)])
+@pytest.mark.parametrize("precision,sig_tol,rgb_tol", [("fp32", 2e-3, 2e-4), ("exact", 2e-2, 2e-3), ("exact_cf", 2e-2, 2e-3)])
 @pytest.mark.parametrize("tag", ["syn", "tkd", "walk"])
 def test_networks(tag, precision, sig_tol, rgb_tol):
     """SpaceNet / MotionNet on explicit points vs the reference modules (raw logits: sigma reaches ~1e3, so the
