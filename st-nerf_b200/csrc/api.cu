@@ -968,10 +968,11 @@ int stnerf_positional_encoding(const float* x, int64_t P, int dim, int n_freq, f
 
 int stnerf_spacenet(stnerf_handle c, int layer, int fine, const float* pos, const float* dirs, const float* times,
                     int64_t P, float* rgb, float* sigma, void* stream) {
-  if (!c || !pos || !dirs || !rgb || !sigma || layer < 0 || layer >= c->l || (fine != 0 && fine != 1)) return STNERF_EINVAL;
+  if (!c || P < 0 || layer < 0 || layer >= c->l || (fine != 0 && fine != 1)) return STNERF_EINVAL;
   SpaceNetDev& net = c->space[fine][layer];
   if (!net.loaded) return STNERF_ENOWEIGHTS;
-  if (net.w.use_time && !times) return STNERF_EINVAL;
+  if (P == 0) return STNERF_OK;        // an empty batch has no buffers (an empty torch tensor's data pointer is null)
+  if (!pos || !dirs || !rgb || !sigma || (net.w.use_time && !times)) return STNERF_EINVAL;
   PointSrc s;
   memset(&s, 0, sizeof(s));
   s.mode = SRC_EXPLICIT; s.pos = pos; s.dirs = dirs; s.times = times; s.pos_stride = 3; s.time_stride = 1;
@@ -991,11 +992,13 @@ __global__ void any_fraction_kernel(const float* __restrict__ xyzt, long long P,
 
 extern "C" int stnerf_motionnet(stnerf_handle c, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
                                 void* stream) {
-  if (!c || !xyzt || !flow || layer < 1 || layer >= c->l || lerp_mode < -1 || lerp_mode > 1) return STNERF_EINVAL;
+  if (!c || P < 0 || layer < 1 || layer >= c->l || lerp_mode < -1 || lerp_mode > 1) return STNERF_EINVAL;
   MotionNetDev& net = c->motion[layer];
   if (!net.loaded) return STNERF_ENOWEIGHTS;
+  if (P == 0) return STNERF_OK;        // see stnerf_spacenet
+  if (!xyzt || !flow) return STNERF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
-  if (lerp_mode < 0 && P > 0) {
+  if (lerp_mode < 0) {
     STNERF_CUDA(cudaMemsetAsync(c->any_frac, 0, 4, st));
     any_fraction_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(xyzt, P, c->any_frac);
     STNERF_LAUNCH_CHECK();
