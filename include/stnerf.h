@@ -206,6 +206,34 @@ int stnerf_spacenet(stnerf_handle h, int layer, int fine, const float* pos, cons
 int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
                      void* stream);
 
+/* ---- training: differentiable SpaceNet / MotionNet in fp32 on CUDA cores (no context) ------------------------------------
+ * `weights` is a DEVICE blob in the stnerf_load_* order above (state_dict order, nn.Linear (out,in) row-major), read in place;
+ * `d_weights` receives the gradient of every tensor in the same order and size (464260 / 466948 / 77315 floats).
+ * A training forward fills `saved` (stnerf_train_saved_floats floats) with what the backward of the same points needs: the
+ * encodings and the post-ReLU activations, feature-major.  `scratch` is stnerf_train_scratch_bytes bytes of device memory the
+ * call may overwrite.  Products and sums are fp32; the forward's outputs are bit-identical to STNERF_PREC_FP32_SIMT.  Weight
+ * and bias gradients are sums over the points in an order fixed by P alone (no atomics): identical calls, identical bits.
+ * P = 0 succeeds (a backward then zeroes d_weights); P < 0 and missing required pointers return STNERF_EINVAL.
+ * kind: 0 = SpaceNet, 1 = MotionNet; use_time: the SpaceNet's rgb head consumes PE(time) (rgb_net.1 width 304).          */
+size_t stnerf_train_saved_floats(int kind, int use_time, int64_t P);
+size_t stnerf_train_scratch_bytes(int kind, int use_time, int64_t P);
+/* modeling/spacenet.py:101-160 (bins mode and maxs/mins are the caller's).  pos, dirs (P,3), times (P) | NULL -> rgb (P,3),
+ * sigma (P) raw. */
+int stnerf_spacenet_train_forward(const float* weights, int use_time, const float* pos, const float* dirs, const float* times,
+                                  int64_t P, float* rgb, float* sigma, float* saved, void* stream);
+/* Gradient of spacenet.py:101-160 for d_rgb (P,3), d_sigma (P): d_weights, and d_pos (P,3) through the encoding of
+ * utils/dimension_kernel.py:24-33 and both of its uses (:135, the skip concatenation :137), or d_pos = NULL for none.
+ * Directions and times get no gradient (modeling/layered_rfrender.py:272,314-315 detach them). */
+int stnerf_spacenet_backward(const float* weights, int use_time, int64_t P, const float* saved, const float* d_rgb,
+                             const float* d_sigma, float* d_weights, float* d_pos, void* scratch, size_t scratch_bytes,
+                             void* stream);
+/* modeling/motion_net.py:34-71.  xyzt (P,4) -> flow (P,3); lerp_mode as in stnerf_motionnet. */
+int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int64_t P, int lerp_mode, float* flow, float* saved,
+                                   void* scratch, size_t scratch_bytes, void* stream);
+/* Gradient of motion_net.py:34-71 for d_flow (P,3): d_weights only (xyzt is detached, layered_rfrender.py:314-315). */
+int stnerf_motionnet_backward(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
+                              void* scratch, size_t scratch_bytes, void* stream);
+
 /* Packed-weight image (cache next to the checkpoint; replaces re-running the state_dict -> MMA-layout packing that follows
  * render/layered_neural_renderer.py:109-117 `torch.load` + `load_state_dict`).  `export` writes every loaded network's
  * device images (fp32 SIMT layout, fp16 hi/lo tensor-core stream, fp32 bias/head block) into a HOST buffer; with

@@ -73,6 +73,12 @@ _SIGNATURES = {
     "stnerf_positional_encoding": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
     "stnerf_spacenet": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P]),
     "stnerf_motionnet": (C.c_int, [_P, C.c_int, _P, C.c_int64, C.c_int, _P, _P]),
+    "stnerf_train_saved_floats": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "stnerf_train_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "stnerf_spacenet_train_forward": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P, _P]),
+    "stnerf_spacenet_backward": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
+    "stnerf_motionnet_train_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, C.c_size_t, _P]),
+    "stnerf_motionnet_backward": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, _P]),
     "stnerf_debug_read_depths": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P]),
     "stnerf_launch_count": (C.c_uint64, []),
     "stnerf_set_ray_ids": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64]),
