@@ -233,6 +233,13 @@ int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int6
 /* Gradient of motion_net.py:34-71 for d_flow (P,3): d_weights only (xyzt is detached, layered_rfrender.py:314-315). */
 int stnerf_motionnet_backward(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
                               void* scratch, size_t scratch_bytes, void* stream);
+/* Gradient of layers/render_layer.py:8-58 (gen_weight + VolumeRenderer.forward) for stnerf_composite's outputs.
+ * d_color (n,3), d_depth (n), d_acc (n), d_w (n,S): any may be NULL (zero).  -> d_rgb (n,S,3), d_sigma (n,S).
+ * t gets no gradient (the reference detaches every depth it composites, layered_rfrender.py:314,461).
+ * Recomputes the forward from (t, rgb, sigma); deterministic (no atomics).  n = 0 touches no pointer.            */
+int stnerf_composite_backward(const float* t, const float* rgb, const float* sigma, int64_t n, int S, float boarder,
+                              const float* d_color, const float* d_depth, const float* d_acc, const float* d_w,
+                              float* d_rgb, float* d_sigma, void* stream);
 
 /* Packed-weight image (cache next to the checkpoint; replaces re-running the state_dict -> MMA-layout packing that follows
  * render/layered_neural_renderer.py:109-117 `torch.load` + `load_state_dict`).  `export` writes every loaded network's

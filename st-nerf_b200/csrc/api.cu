@@ -1072,4 +1072,14 @@ int stnerf_motionnet_backward(const float* weights, int64_t P, const float* save
   return launch_motionnet_backward(weights, P, saved, d_flow, d_weights, scratch, st);
 }
 
+int stnerf_composite_backward(const float* t, const float* rgb, const float* sigma, int64_t n, int S, float boarder,
+                              const float* d_color, const float* d_depth, const float* d_acc, const float* d_w, float* d_rgb,
+                              float* d_sigma, void* stream) {
+  if (n < 0 || S < 1) return STNERF_EINVAL;
+  if (n == 0) return STNERF_OK;
+  if (!t || !rgb || !sigma || !d_rgb || !d_sigma) return STNERF_EINVAL;
+  return launch_composite_backward(t, rgb, sigma, n, S, boarder, d_color, d_depth, d_acc, d_w, d_rgb, d_sigma,
+                                   (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -189,6 +189,9 @@ struct CompositeArgs {
 int launch_composite_pass(const CompositeArgs& a, const DevScene& scene, int n_layers, cudaStream_t st);
 int launch_composite_simple(const float* t, const float* rgb, const float* sigma, long long n, int S, float boarder,
                             float* color, float* depth, float* acc, float* w, cudaStream_t st);
+int launch_composite_backward(const float* t, const float* rgb, const float* sigma, long long n, int S, float boarder,
+                              const float* d_color, const float* d_depth, const float* d_acc, const float* d_w, float* d_rgb,
+                              float* d_sigma, cudaStream_t st);
 int launch_sample_pdf(const float* t, const float* w, const float* u, long long n, int n1, int n2, float* z,
                       float* t_fine, cudaStream_t st);
 

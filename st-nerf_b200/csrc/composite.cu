@@ -567,6 +567,129 @@ int launch_composite_simple(const float* t, const float* rgb, const float* sigma
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// Gradient of composite_simple_kernel's outputs (color, depth, acc, w) with respect to rgb and sigma.  Warp per ray.
+//   w_k = alpha_k T_k,  T_k = prod_{j<k} f_j,  f_j = 1 - alpha_j + 1e-10,  alpha = 1 - exp(-relu(sigma) delta)
+//   g_k = d_color . sigmoid(rgb_k) + d_depth t_k + d_acc + d_w_k                      (dL/dw_k)
+//   d_alpha_k = T_k g_k - (sum_{m>k} w_m g_m) / f_k                                    (f_k >= 1e-10: never 0)
+//   d_sigma_k = d_alpha_k (delta_k exp(-relu(sigma_k) delta_k)) [sigma_k > 0],   d_rgb_k = d_color w_k y (1 - y)
+// Nothing is saved by the forward: pass 1 recomputes the transmittance at the start of every 32-sample row with the
+// forward's arithmetic (same rows, same scan, so T and w are the forward's bits) into shared memory; pass 2 walks the rows
+// from the last to the first, carrying the suffix sum of w g down with a reverse warp scan.  Every output element is
+// written once by one lane: no atomics, and a ray's gradients do not depend on the rest of the batch.
+// ---------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float warp_incl_add_rev(float v, int lane) {      // sum over lanes >= lane
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const float n = __shfl_down_sync(FULL, v, d);
+    if (lane + d < 32) v = v + n;
+  }
+  return v;
+}
+
+// delta, exp(-relu(sigma) delta), alpha and f of sample j < S of one ray, as composite_simple_kernel computes them
+__device__ __forceinline__ void backward_sample(const float* tp, const float* sp, int S, int j, float boarder, float& tj,
+                                                float& sg, float& delta, float& e, float& alpha, float& f) {
+  tj = __ldg(tp + j);
+  sg = __ldg(sp + j);
+  delta = (j == S - 1) ? boarder : (__ldg(tp + j + 1) - tj);
+  e = expf(-fmaxf(sg, 0.0f) * delta);
+  alpha = 1.0f - e;
+  f = (1.0f - alpha) + 1e-10f;
+}
+
+__global__ void __launch_bounds__(256) composite_backward_kernel(
+    const float* __restrict__ t, const float* __restrict__ rgb, const float* __restrict__ sigma, long long n, int S,
+    float boarder, const float* __restrict__ d_color, const float* __restrict__ d_depth, const float* __restrict__ d_acc,
+    const float* __restrict__ d_w, float* __restrict__ d_rgb, float* __restrict__ d_sigma) {
+  extern __shared__ float s_rows[];
+  const int lane = threadIdx.x & 31;
+  const int rows = (S + 31) >> 5;
+  float* s_carry = s_rows + (size_t)(threadIdx.x >> 5) * rows;      // T at the first sample of every row
+  const long long wid = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long r = wid; r < n; r += nw) {
+    const float* tp = t + r * S;
+    const float* sp = sigma + r * S;
+    const float* cp = rgb + r * S * 3;
+    float carry = 1.0f;
+    for (int row = 0; row < rows; ++row) {
+      const int j = row * 32 + lane;
+      float f = 1.0f;
+      if (j < S) {
+        float tj, sg, delta, e, alpha;
+        backward_sample(tp, sp, S, j, boarder, tj, sg, delta, e, alpha, f);
+      }
+      const float incl = warp_incl_mul(f, lane);
+      if (lane == 0) s_carry[row] = carry;
+      carry = carry * __shfl_sync(FULL, incl, 31);
+    }
+    __syncwarp();
+    const float dcr = d_color ? __ldg(d_color + 3 * r) : 0.0f;
+    const float dcg = d_color ? __ldg(d_color + 3 * r + 1) : 0.0f;
+    const float dcb = d_color ? __ldg(d_color + 3 * r + 2) : 0.0f;
+    const float dd = d_depth ? __ldg(d_depth + r) : 0.0f;
+    const float da = d_acc ? __ldg(d_acc + r) : 0.0f;
+    float later_rows = 0.0f;                 // sum of w_m g_m over the rows after this one
+    for (int row = rows - 1; row >= 0; --row) {
+      const int j = row * 32 + lane;
+      const bool valid = j < S;
+      float tj = 0.f, sg = 0.f, delta = 0.f, e = 1.f, alpha = 0.f, f = 1.f;
+      float y0 = 0.f, y1 = 0.f, y2 = 0.f, g = 0.f;
+      if (valid) {
+        backward_sample(tp, sp, S, j, boarder, tj, sg, delta, e, alpha, f);
+        if (d_color) {
+          y0 = sigmoidf_ref(__ldg(cp + 3 * j));
+          y1 = sigmoidf_ref(__ldg(cp + 3 * j + 1));
+          y2 = sigmoidf_ref(__ldg(cp + 3 * j + 2));
+          g = dcr * y0 + dcg * y1 + dcb * y2;
+        }
+        if (d_depth) g = g + dd * tj;       // NULL upstreams add nothing (not 0 * t: t may be huge)
+        if (d_acc) g = g + da;
+        if (d_w) g = g + __ldg(d_w + r * S + j);
+      }
+      const float incl = warp_incl_mul(f, lane);
+      float excl = __shfl_up_sync(FULL, incl, 1);
+      if (lane == 0) excl = 1.0f;
+      const float T = s_carry[row] * excl;
+      const float w = alpha * T;
+      const float sfx = warp_incl_add_rev(valid ? w * g : 0.0f, lane);
+      float after = __shfl_down_sync(FULL, sfx, 1);
+      if (lane == 31) after = 0.0f;
+      const float later = later_rows + after;
+      later_rows = later_rows + __shfl_sync(FULL, sfx, 0);
+      if (valid) {
+        const float dalpha = T * g - later / f;
+        d_sigma[r * S + j] = sg > 0.0f ? dalpha * (delta * e) : 0.0f;     // torch's relu: no gradient at exactly 0
+        float* o = d_rgb + (r * S + j) * 3;
+        o[0] = dcr * w * (1.0f - y0) * y0;
+        o[1] = dcg * w * (1.0f - y1) * y1;
+        o[2] = dcb * w * (1.0f - y2) * y2;
+      }
+    }
+    __syncwarp();
+  }
+}
+
+int launch_composite_backward(const float* t, const float* rgb, const float* sigma, long long n, int S, float boarder,
+                              const float* d_color, const float* d_depth, const float* d_acc, const float* d_w, float* d_rgb,
+                              float* d_sigma, cudaStream_t st) {
+  if (n <= 0) return STNERF_OK;
+  const size_t per_warp = (size_t)((S + 31) / 32) * sizeof(float);
+  int wpb = 8;
+  while (wpb > 1 && per_warp * wpb > 48 * 1024) wpb >>= 1;
+  const size_t smem = per_warp * wpb;
+  if (smem > 200 * 1024) return STNERF_EINVAL;                  // more than 1.6 M samples per ray
+  if (smem > 48 * 1024)
+    STNERF_CUDA(cudaFuncSetAttribute(composite_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  long long blocks = (n + wpb - 1) / wpb;
+  if (blocks > (long long)device_sms() * 64 / wpb) blocks = (long long)device_sms() * 64 / wpb;
+  composite_backward_kernel<<<(int)blocks, wpb * 32, smem, st>>>(t, rgb, sigma, n, S, boarder, d_color, d_depth, d_acc, d_w,
+                                                                 d_rgb, d_sigma);
+  STNERF_LAUNCH_CHECK();
+  return STNERF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // Unit entry point a11: sample_pdf (+ optional sort-merge with the coarse depths).
 // ---------------------------------------------------------------------------------------------------------
 __global__ void sample_pdf_kernel(const float* __restrict__ t, const float* __restrict__ w, const float* __restrict__ u,

@@ -14,6 +14,7 @@ from .pose_renderer import PoseRenderer
 from .camera_path import CameraPath
 from . import checkpoint_io
 from . import nets
+from . import volume
 
 __all__ = ["LayeredRFRender", "build_layered_model", "fresh_state_dict", "NativeRenderer", "StnerfError", "ops",
-           "launch_count", "split_planes", "PoseRenderer", "CameraPath", "checkpoint_io", "nets"]
+           "launch_count", "split_planes", "PoseRenderer", "CameraPath", "checkpoint_io", "nets", "volume"]
