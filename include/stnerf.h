@@ -241,6 +241,39 @@ int stnerf_composite_backward(const float* t, const float* rgb, const float* sig
                               const float* d_color, const float* d_depth, const float* d_acc, const float* d_w,
                               float* d_rgb, float* d_sigma, void* stream);
 
+/* ---- training: the per-sample work of a differentiable LayeredRFRender.forward around the networks ------------------------
+ * (modeling/layered_rfrender.py:141-734 as stnerf_render computes it; the networks are the stnerf_*_train_* calls above and the
+ * compositing is stnerf_composite / stnerf_composite_backward / stnerf_sample_pdf.)  Every call uses the context's scene
+ * (stnerf_set_scene) and box table; n = 0 succeeds; bad arguments return STNERF_EINVAL.                                      */
+/* layers/RaySamplePoint.py:8-107 for every layer (the sampling of stnerf_render, jitter (l,n,n1) or NULL = Philox stream i
+ * with `seed`) -> t (l,n,n1), mask (l,n) uint8, and, per performer layer i >= 1, hit[i*n + j] = the j-th ray whose box was hit
+ * in ASCENDING ray order (the boolean index `[ray_mask[i]]` of :343-356 / :400-413; block counts, an exclusive scan, then the
+ * writes -- deterministic, unlike the render's block-claimed lists).  hit_counts_host[i] = the number of hit rays (n for
+ * layer 0), any_frac_host[i] = 1 iff a hit ray's frame id of layer i is fractional (modeling/motion_net.py:53).  HOST
+ * arrays of l ints: the call copies them back and synchronizes `stream` once -- they size the saved activations.          */
+int stnerf_train_sample(stnerf_handle h, const float* rays, int64_t n, int ray_stride, int n1, const float* jitter, uint64_t seed,
+                        float* t, uint8_t* mask, int32_t* hit, int32_t* hit_counts_host, int32_t* any_frac_host, void* stream);
+/* The network inputs of one layer and pass in hit order (layered_rfrender.py:293-303 + :340-356 + :397-413 coarse,
+ * :465-475 + :495-510 + :552-566 fine): m rays (hit == NULL and m = n for the background, else the hit list of the layer),
+ * S depths each in t (n,S).  Point j*S+k: pos = t*d + o with the pass' inverse edit, rounded as stnerf_render rounds it
+ * (bit-identical); dirs = d; times = frame-id column 6+layer (6 for 7-column rays); xyzt = (pos, time), MotionNet's input.
+ * Any output may be NULL.                                                                                                    */
+int stnerf_train_points(stnerf_handle h, int layer, int fine, const float* rays, int64_t n, int ray_stride, const float* t, int S,
+                        const int32_t* hit, int64_t m, float* pos, float* dirs, float* times, float* xyzt, void* stream);
+/* `rgbs[i][idx] = ...; density[i][idx] = ...` with the pass' density masks (layered_rfrender.py:412-422 coarse: t < 0 for a
+ * performer, t < near for the background, the thresholds when the scene applies them; :538-547 / :564-576 fine: thresholds,
+ * alpha on layer 2).  Compact rgb_c (m*S,3), sigma_c (m*S) in hit order -> dense rgb (n,S,3), sigma (n,S), zeros for rays
+ * not in the list, and factor (m*S): 0 where masked, the alpha factor, or 1 -- what stnerf_train_gather multiplies by.    */
+int stnerf_train_scatter(stnerf_handle h, int layer, int fine, const float* t, int64_t n, int S, const int32_t* hit, int64_t m,
+                         const float* rgb_c, const float* sigma_c, float* rgb, float* sigma, float* factor, void* stream);
+/* Backward of stnerf_train_scatter: d_rgb (n,S,3), d_sigma (n,S) (either may be NULL = zero) -> d_rgb_c (m*S,3),
+ * d_sigma_c (m*S) = d_sigma * factor, in hit order.  A masked sample gets a zero gradient, as torch gives `density[mask] = 0`. */
+int stnerf_train_gather(stnerf_handle h, int S, const int32_t* hit, int64_t m, const float* factor, const float* d_rgb,
+                        const float* d_sigma, float* d_rgb_c, float* d_sigma_c, void* stream);
+/* utils/sample_pdf.py:31 without injected uniforms: u (l,n,n2) = the Philox draws stnerf_render makes for the fine resampling
+ * with this seed (stream 64+layer, keyed by the ray id), so a training forward places the render's fine samples.             */
+int stnerf_train_uniforms(stnerf_handle h, int64_t n, int n2, uint64_t seed, float* u, void* stream);
+
 /* Packed-weight image (cache next to the checkpoint; replaces re-running the state_dict -> MMA-layout packing that follows
  * render/layered_neural_renderer.py:109-117 `torch.load` + `load_state_dict`).  `export` writes every loaded network's
  * device images (fp32 SIMT layout, fp16 hi/lo tensor-core stream, fp32 bias/head block) into a HOST buffer; with

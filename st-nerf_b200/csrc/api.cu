@@ -1082,4 +1082,95 @@ int stnerf_composite_backward(const float* t, const float* rgb, const float* sig
                                    (cudaStream_t)stream);
 }
 
+// ---- training: the per-sample work around the networks (train_march.cu) ------------------------------------------------------
+static int on_ctx_device(stnerf_ctx* c) {          // the context's scene and weights live on the device it was created on
+  int cur = -1;
+  STNERF_CUDA(cudaGetDevice(&cur));
+  return cur == c->device ? STNERF_OK : STNERF_EINVAL;
+}
+
+static int train_ready(stnerf_ctx* c, int ray_stride) {
+  if (!c->have_scene) return STNERF_EINVAL;
+  int rc = on_ctx_device(c);
+  if (rc) return rc;
+  if (ray_stride < 6 + (c->scene.shared_frame_id ? 1 : c->l)) return STNERF_EINVAL;
+  return STNERF_OK;
+}
+
+int stnerf_train_sample(stnerf_handle c, const float* rays, int64_t n, int ray_stride, int n1, const float* jitter, uint64_t seed,
+                        float* t, uint8_t* mask, int32_t* hit, int32_t* hit_counts_host, int32_t* any_frac_host, void* stream) {
+  if (!c || n < 0 || n1 < 3 || n1 > STNERF_MAX_N1 || !hit_counts_host || !any_frac_host) return STNERF_EINVAL;
+  if ((long long)n * STNERF_MAX_S >= (1LL << 31)) return STNERF_EINVAL;      // 32-bit sample indices, as for a render chunk
+  int rc = train_ready(c, ray_stride);
+  if (rc) return rc;
+  hit_counts_host[0] = (int32_t)n;
+  any_frac_host[0] = 0;
+  for (int i = 1; i < c->l; ++i) hit_counts_host[i] = any_frac_host[i] = 0;
+  if (n == 0) return STNERF_OK;
+  if (!rays || !t || !mask || !hit) return STNERF_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t ints = 2 * STNERF_MAX_LAYERS + train_hits_scratch_ints(n, c->l);
+  int* scratch = nullptr;
+  STNERF_CUDA(cudaMallocAsync((void**)&scratch, ints * sizeof(int), st));
+  int* counts = scratch;                              // sample_kernel's own (unordered) counters, then the ordered totals
+  int* lerp = scratch + STNERF_MAX_LAYERS;
+  STNERF_CUDA(cudaMemsetAsync(scratch, 0, 2 * STNERF_MAX_LAYERS * sizeof(int), st));
+  // sampling as in render_core; its block-ordered hit lists land in `hit` and are overwritten in ray order below
+  rc = launch_sample(rays, n, ray_stride, c->dscene, c->l, n1, jitter, n * n1, seed, 0, c->idmap, t, n * n1, mask, n, hit, n,
+                     counts, lerp, st, c->box_table, c->box_frames);
+  if (!rc) rc = launch_train_hits(mask, n, c->l, rays, ray_stride, c->scene.shared_frame_id, hit,
+                                  scratch + 2 * STNERF_MAX_LAYERS, counts, st);
+  int host[2 * STNERF_MAX_LAYERS];
+  if (!rc && cudaMemcpyAsync(host, counts, sizeof(host), cudaMemcpyDeviceToHost, st) != cudaSuccess) rc = STNERF_ECUDA;
+  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = STNERF_ECUDA;     // the one host sync: sizes the saved activations
+  cudaFreeAsync(scratch, st);
+  if (rc) return rc;
+  for (int i = 1; i < c->l; ++i) { hit_counts_host[i] = host[i]; any_frac_host[i] = host[STNERF_MAX_LAYERS + i]; }
+  return STNERF_OK;
+}
+
+int stnerf_train_points(stnerf_handle c, int layer, int fine, const float* rays, int64_t n, int ray_stride, const float* t, int S,
+                        const int32_t* hit, int64_t m, float* pos, float* dirs, float* times, float* xyzt, void* stream) {
+  if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || n < 0 || m < 0 || S < 1 || S > STNERF_MAX_S) return STNERF_EINVAL;
+  if ((layer == 0) != (hit == nullptr) || m > n || (layer == 0 && m != n)) return STNERF_EINVAL;
+  int rc = train_ready(c, ray_stride);
+  if (rc) return rc;
+  if (m == 0) return STNERF_OK;
+  if (!rays || !t || (!pos && !dirs && !times && !xyzt)) return STNERF_EINVAL;
+  PointSrc s;
+  memset(&s, 0, sizeof(s));
+  s.mode = SRC_MARCH; s.rays = rays; s.ray_stride = ray_stride; s.t = t; s.S = S; s.hit = hit; s.n_slots = m;
+  s.layer = c->scene.shared_frame_id ? 0 : layer;
+  fill_edit(s, c->scene, layer, fine != 0);
+  return launch_train_points(s, (long long)m * S, pos, dirs, times, xyzt, (cudaStream_t)stream);
+}
+
+int stnerf_train_scatter(stnerf_handle c, int layer, int fine, const float* t, int64_t n, int S, const int32_t* hit, int64_t m,
+                         const float* rgb_c, const float* sigma_c, float* rgb, float* sigma, float* factor, void* stream) {
+  if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || n < 0 || m < 0 || m > n || S < 1) return STNERF_EINVAL;
+  if ((layer == 0) != (hit == nullptr) || (layer == 0 && m != n) || !c->have_scene) return STNERF_EINVAL;
+  const int rc = on_ctx_device(c);
+  if (rc) return rc;
+  if (n == 0) return STNERF_OK;
+  if (!t || !rgb || !sigma || (m > 0 && (!rgb_c || !sigma_c || !factor))) return STNERF_EINVAL;
+  return launch_train_scatter(c->dscene, layer, fine, t, n, S, hit, m * S, rgb_c, sigma_c, rgb, sigma, factor, (cudaStream_t)stream);
+}
+
+int stnerf_train_gather(stnerf_handle c, int S, const int32_t* hit, int64_t m, const float* factor, const float* d_rgb,
+                        const float* d_sigma, float* d_rgb_c, float* d_sigma_c, void* stream) {
+  if (!c || m < 0 || S < 1) return STNERF_EINVAL;
+  const int rc = on_ctx_device(c);
+  if (rc) return rc;
+  if (m == 0) return STNERF_OK;
+  if (!factor || !d_rgb_c || !d_sigma_c) return STNERF_EINVAL;
+  return launch_train_gather(S, hit, m * S, factor, d_rgb, d_sigma, d_rgb_c, d_sigma_c, (cudaStream_t)stream);
+}
+
+int stnerf_train_uniforms(stnerf_handle c, int64_t n, int n2, uint64_t seed, float* u, void* stream) {
+  if (!c || n < 0 || n2 < 0) return STNERF_EINVAL;
+  if (n == 0 || n2 == 0) return STNERF_OK;
+  if (!u) return STNERF_EINVAL;
+  return launch_train_uniforms(n, n2, c->l, seed, c->idmap, u, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -92,6 +92,21 @@ struct PointSrc {
   float shift[3], scale, pivot[3];
 };
 
+// A marched sample p = t*d + o with separately rounded product and sum (layers/RaySamplePoint.py:103,
+// layered_rfrender.py:465), then the inverse edit of the pass (:293-303 / :467-475).  rp = the ray (o at 0..2), d = its
+// direction.  Shared by the SIMT networks' SRC_MARCH fetch and the training point assembly, so both round alike.
+__device__ __forceinline__ void march_point(const PointSrc& s, const float* rp, float tt, float dx, float dy, float dz,
+                                            float v[3]) {
+  v[0] = __fadd_rn(__fmul_rn(tt, dx), rp[0]);
+  v[1] = __fadd_rn(__fmul_rn(tt, dy), rp[1]);
+  v[2] = __fadd_rn(__fmul_rn(tt, dz), rp[2]);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if (s.shift_on) v[a] = __fsub_rn(v[a], s.shift[a]);                                        // :298 / :471
+    if (s.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], s.pivot[a]), s.scale), s.pivot[a]);   // :303 / :475
+  }
+}
+
 __device__ __forceinline__ long long src_num_points(const PointSrc& s) {
   long long slots = s.count ? (long long)(*s.count) : s.n_slots;
   return slots * (long long)s.S;
@@ -213,5 +228,17 @@ int launch_motionnet_train_forward(const float* W, const float* xyzt, long long 
                                    float* flow, float* saved, cudaStream_t st);
 int launch_motionnet_backward(const float* W, long long P, const float* saved, const float* d_flow, float* dW, void* scratch,
                               cudaStream_t st);
+
+// train_march.cu (the per-sample work of a training step around the networks)
+size_t train_hits_scratch_ints(long long n, int n_layers);
+// totals_frac: [STNERF_MAX_LAYERS] hit counts then [STNERF_MAX_LAYERS] "any fractional frame id" flags (performer layers)
+int launch_train_hits(const uint8_t* mask, long long n, int n_layers, const float* rays, int ray_stride, int fid_shared, int* hit,
+                      int* scratch, int* totals_frac, cudaStream_t st);
+int launch_train_points(const PointSrc& s, long long P, float* pos, float* dirs, float* times, float* xyzt, cudaStream_t st);
+int launch_train_scatter(const DevScene& sc, int layer, int fine, const float* t, long long n, int S, const int* hit, long long P,
+                         const float* rgb_c, const float* sigma_c, float* rgb, float* sigma, float* factor, cudaStream_t st);
+int launch_train_gather(int S, const int* hit, long long P, const float* factor, const float* d_rgb, const float* d_sigma,
+                        float* d_rgb_c, float* d_sigma_c, cudaStream_t st);
+int launch_train_uniforms(long long n, int n2, int n_layers, uint64_t seed, RayIdMap idmap, float* u, cudaStream_t st);
 
 }  // namespace stnerf

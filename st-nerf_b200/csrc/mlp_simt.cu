@@ -111,14 +111,8 @@ __device__ __forceinline__ TilePoint fetch_point(const PointSrc& s, long long p,
     return q;
   }
   const float tt = s.t[ray * s.S + k];
-  // p = t*d + o with separately rounded product and sum (layers/RaySamplePoint.py:103, layered_rfrender.py:465)
-  float v[3] = {__fadd_rn(__fmul_rn(tt, q.dx), rp[0]), __fadd_rn(__fmul_rn(tt, q.dy), rp[1]),
-                __fadd_rn(__fmul_rn(tt, q.dz), rp[2])};
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    if (s.shift_on) v[a] = __fsub_rn(v[a], s.shift[a]);                                        // :298 / :471
-    if (s.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], s.pivot[a]), s.scale), s.pivot[a]);   // :303 / :475
-  }
+  float v[3];
+  march_point(s, rp, tt, q.dx, q.dy, q.dz, v);      // common.cuh (also the training point assembly, train_march.cu)
   q.x = v[0]; q.y = v[1]; q.z = v[2];
   return q;
 }

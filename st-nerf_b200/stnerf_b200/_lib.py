@@ -80,6 +80,12 @@ _SIGNATURES = {
     "stnerf_motionnet_train_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, C.c_size_t, _P]),
     "stnerf_motionnet_backward": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, _P]),
     "stnerf_composite_backward": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P, _P, _P, _P, _P, _P]),
+    "stnerf_train_sample": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, C.c_uint64, _P, _P, _P, _P, _P, _P]),
+    "stnerf_train_points": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P, C.c_int, _P, C.c_int64, _P, _P, _P, _P,
+                                      _P]),
+    "stnerf_train_scatter": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),
+    "stnerf_train_gather": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),
+    "stnerf_train_uniforms": (C.c_int, [_P, C.c_int64, C.c_int, C.c_uint64, _P, _P]),
     "stnerf_debug_read_depths": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P]),
     "stnerf_launch_count": (C.c_uint64, []),
     "stnerf_set_ray_ids": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64]),

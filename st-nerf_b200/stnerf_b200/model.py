@@ -267,8 +267,9 @@ class LayeredRFRender(torch.nn.Module):
         return self._native
 
     # ---- forward (layered_rfrender.py:141) ---------------------------------------------------------------------
-    def forward(self, rays, labels=None, bboxes=None, only_coarse=False, near_far=None, near_far_points=[],
-                density_threshold=0.0001, bkgd_density_threshold=0):
+    def _prologue(self, rays, density_threshold, bkgd_density_threshold):
+        """Ray-layout parse, scene constants and box table of one forward (layered_rfrender.py:151-242) on the context.
+        Returns the context and the rays as detached fp32."""
         l = self.layer_num + 1
         width = rays.size(-1)
         if width == 7 + self.layer_num:
@@ -301,6 +302,12 @@ class LayeredRFRender(torch.nn.Module):
         elif getattr(self, "_table_key", None) is not None:
             nat.set_box_table(None)
             self._table_key = None
+        return nat, rays
+
+    def forward(self, rays, labels=None, bboxes=None, only_coarse=False, near_far=None, near_far_points=[],
+                density_threshold=0.0001, bkgd_density_threshold=0):
+        l = self.layer_num + 1
+        nat, rays = self._prologue(rays, density_threshold, bkgd_density_threshold)
         jitter, u = self._inject if self._inject is not None else (None, None)
         self._inject = None
         self.seed += 1
@@ -314,5 +321,9 @@ class LayeredRFRender(torch.nn.Module):
 
 
 def build_layered_model(cfg, camera_num=0, scale=None, shift=None):
-    """modeling/__init__.py:5-7."""
+    """modeling/__init__.py:5-7.  cfg.MODEL.B200_TRAINABLE (default False) selects the trainable model
+    (stnerf_b200.train.TrainableLayeredRFRender): network parameters, a differentiable forward."""
+    if bool(getattr(cfg.MODEL, "B200_TRAINABLE", False)):
+        from .train import TrainableLayeredRFRender
+        return TrainableLayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift)
     return LayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift)
