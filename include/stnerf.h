@@ -195,6 +195,23 @@ int stnerf_composite(const float* t, const float* rgb, const float* sigma, int64
  * t (n,n1), w (n,n1) full weights (the [1:-1] slice is taken inside), u (n,n2) -> z (n,n2)|NULL, t_fine (n,n1+n2)|NULL */
 int stnerf_sample_pdf(const float* t, const float* w, const float* u, int64_t n, int n1, int n2,
                       float* z, float* t_fine, void* stream);
+/* One compositing pass of stnerf_render on explicit network outputs: the density masks of modeling/layered_rfrender.py:412-422
+ * (coarse) / :538-547, 564-576 (fine), every hit layer's own VolumeRenderer.forward, the depth-ordered merge of :425-448 /
+ * :587-606 and, in a coarse pass with n2 > 0, sample_pdf + the sort of :459-463 -- the kernel the render path launches, with
+ * no context.  Uses near_plane, the thresholds, alpha_layer2, boarder_weight and shown[] of `scene_host`.
+ * t (l,n,S), raw (l,n,S,4) = rgb logits + raw sigma, mask (l,n) uint8 (row 0 is ignored: the background is always hit; may be
+ * NULL when l = 1), u (l,n,n2) or NULL = Philox stream 64+layer of `seed`, keyed by the ray index.
+ * fine = 0: 3 <= S <= STNERF_MAX_N1, n2 >= 0, S + n2 <= STNERF_MAX_S;  fine = 1: 1 <= S <= STNERF_MAX_S, n2 = 0.
+ * images (l+1, 5n): image 0 merged, 1+i layer i; pixel_layout 0 = rgb (n,3) | depth (n) | acc (n), 1 = (n,5) interleaved.
+ *   NULL with n2 > 0: the pass only resamples.  A layer the ray misses gets a zero pixel.
+ * t_fine (l,n,S+n2): sort(cat(t, z)) of every HIT (ray, layer); rows of missed layers are not written.  Required iff n2 > 0.
+ * z_new (l,n,n2) ascending new depths and src_map (l,n,S+n2) the origin of every fine depth (k < S: coarse sample k, S + e:
+ *   new depth e): both or neither, and only where the register-resident resampling runs and an origin fits a byte
+ *   (S + n2 <= 256, n2 <= 256); STNERF_EINVAL elsewhere.  With STNERF_PASS_GENERIC=1 in the environment a coarse pass takes the
+ *   shared-memory path whatever its sample counts (the path of n2 > 256), which writes t_fine only.                       */
+int stnerf_composite_pass(const stnerf_scene* scene_host, int n_layers, int fine, const float* t, const float* raw,
+                          const uint8_t* mask, const float* u, uint64_t seed, int64_t n, int S, int n2, int pixel_layout,
+                          float* images, float* t_fine, float* z_new, uint8_t* src_map, void* stream);
 /* utils/dimension_kernel.py:24-33.  x (P,dim) -> out (P, dim*(1+2*n_freq)) */
 int stnerf_positional_encoding(const float* x, int64_t P, int dim, int n_freq, float* out, void* stream);
 /* modeling/spacenet.py:101-160.  pos (P,3), dirs (P,3), times (P)|NULL -> rgb (P,3) raw, sigma (P) raw.
@@ -294,9 +311,12 @@ int stnerf_selftest_umma_accum(int reps, float* max_err_host, float* mean_signed
 
 /* Diagnostic read-back of the sample depths of the LAST chunk rendered by stnerf_render (parity tooling: which depths did
  * utils/sample_pdf.py:18-63 + the sort of modeling/layered_rfrender.py:462 produce for these rays?).
- * what = 0: coarse depths of `layer`, (n_rays, n1);  what = 1: fine depths, (n_rays, n1+n2).  dst is a DEVICE buffer of
- * n_rays*S floats; n_rays must not exceed the rays of that chunk and S must be the sample count of that call.          */
-int stnerf_debug_read_depths(stnerf_handle h, int what, int layer, float* dst, int64_t n_rays, int S, void* stream);
+ * what = 0: coarse depths of `layer`, (n_rays, n1) floats;  what = 1: fine depths, (n_rays, n1+n2) floats;  what = 2: the new
+ * depths in ascending order, (n_rays, n2) floats;  what = 3: the origin of every fine depth, (n_rays, n1+n2) BYTES (k < n1:
+ * coarse sample k, n1 + e: new depth e) -- 2 and 3 exist only when that render reused the coarse pass' flow in the fine pass
+ * (a tensor-core mode, n1 + n2 <= 256), STNERF_EINVAL otherwise.  dst is a DEVICE buffer of n_rays*S elements; n_rays must not
+ * exceed the rays of that chunk and S must be the row length named above.  Rows of rays that miss `layer` are stale.      */
+int stnerf_debug_read_depths(stnerf_handle h, int what, int layer, void* dst, int64_t n_rays, int S, void* stream);
 
 /* Number of kernels this library has launched since load (bench.py's gpu_launches claim). */
 uint64_t stnerf_launch_count(void);

@@ -48,6 +48,7 @@ struct stnerf_ctx {
   int cap_n1 = 0, cap_s2 = 0;
   long long last_chunk_rays = 0;       // geometry of the most recent chunk (stnerf_debug_read_depths)
   int last_n1 = 0, last_s2 = 0;
+  bool last_reuse = false;             // that chunk's coarse pass wrote z_new / src_map
   float *t_coarse = nullptr, *raw_coarse = nullptr, *t_fine = nullptr, *raw_fine = nullptr, *xyz = nullptr;
   // flow reuse (fine pass): per performer layer the coarse pass' deformed points, the new depths and the origin map of t_fine
   float *xyz_coarse = nullptr, *z_new = nullptr;
@@ -429,22 +430,25 @@ int stnerf_weights_import(stnerf_handle c, const void* buf, size_t bytes) {
   return STNERF_OK;
 }
 
+// the scene constants of `l` layers as the kernels read them
+static void dev_scene_from(const stnerf_scene& s, int l, DevScene& d) {
+  memset(&d, 0, sizeof(d));
+  for (int i = 0; i < l; ++i) {
+    for (int a = 0; a < 3; ++a) { d.bmin[i][a] = s.bmin[i][a]; d.bmax[i][a] = s.bmax[i][a]; }
+    d.shown[i] = s.shown[i];
+  }
+  d.near_plane = s.near_plane; d.alpha2 = s.alpha_layer2;
+  d.thr_layer = s.density_threshold; d.thr_bkgd = s.bkgd_density_threshold;
+  d.boarder = s.boarder_weight; d.apply_thr = s.apply_thresholds; d.n_layers = l;
+  d.fid_shared = s.shared_frame_id;
+}
+
 int stnerf_set_scene(stnerf_handle c, const stnerf_scene* s) {
   if (!c || !s) return STNERF_EINVAL;
   c->scene = *s;
-  DevScene& d = c->dscene;
-  memset(&d, 0, sizeof(d));
-  for (int i = 0; i < c->l; ++i) {
-    for (int a = 0; a < 3; ++a) { d.bmin[i][a] = s->bmin[i][a]; d.bmax[i][a] = s->bmax[i][a]; }
-    d.shown[i] = s->shown[i];
-    if (s->scale_coarse_on[i] || s->scale_fine_on[i]) {
-      if (s->scale[i] == 0.0f) return STNERF_EINVAL;
-    }
-  }
-  d.near_plane = s->near_plane; d.alpha2 = s->alpha_layer2;
-  d.thr_layer = s->density_threshold; d.thr_bkgd = s->bkgd_density_threshold;
-  d.boarder = s->boarder_weight; d.apply_thr = s->apply_thresholds; d.n_layers = c->l;
-  d.fid_shared = s->shared_frame_id;
+  dev_scene_from(*s, c->l, c->dscene);
+  for (int i = 0; i < c->l; ++i)
+    if ((s->scale_coarse_on[i] || s->scale_fine_on[i]) && s->scale[i] == 0.0f) return STNERF_EINVAL;
   c->have_scene = true;
   return STNERF_OK;
 }
@@ -628,6 +632,7 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
     // Flow reuse: the merge (fused or stand-alone register path) also writes the new depths and the origin of every fine depth, so
     // the fine pass runs the MotionNet on the n2 new depths only (same network, same points for the other n1: SURVEY A.6).
     const bool reuse = n2 > 0 && c->precision != STNERF_PREC_FP32_SIMT && n1 <= 128 && n2 <= 256 && S2 <= 256 && !c->no_reuse;
+    c->last_reuse = reuse;
     FuseCoarse ft;
     memset(&ft, 0, sizeof(ft));
     if (fuse) {
@@ -868,13 +873,19 @@ int stnerf_render_views_host(stnerf_handle c, const stnerf_view* views_host, int
   return STNERF_OK;
 }
 
-int stnerf_debug_read_depths(stnerf_handle c, int what, int layer, float* dst, int64_t n_rays, int S, void* stream) {
-  if (!c || !dst || layer < 0 || layer >= c->l || n_rays < 0 || (what != 0 && what != 1)) return STNERF_EINVAL;
+int stnerf_debug_read_depths(stnerf_handle c, int what, int layer, void* dst, int64_t n_rays, int S, void* stream) {
+  if (!c || !dst || layer < 0 || layer >= c->l || n_rays < 0 || what < 0 || what > 3) return STNERF_EINVAL;
   if (!c->t_coarse || n_rays > c->last_chunk_rays) return STNERF_EINVAL;
-  if (S != (what ? c->last_s2 : c->last_n1)) return STNERF_EINVAL;
-  const long long R = c->chunk_rays;
-  const float* src = what ? c->t_fine + (size_t)layer * R * c->cap_s2 : c->t_coarse + (size_t)layer * R * c->cap_n1;
-  STNERF_CUDA(cudaMemcpyAsync(dst, src, (size_t)n_rays * S * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (what >= 2 && !c->last_reuse) return STNERF_EINVAL;
+  const int n2 = c->last_s2 - c->last_n1;
+  if (S != (what == 0 ? c->last_n1 : what == 2 ? n2 : c->last_s2)) return STNERF_EINVAL;
+  const size_t R = (size_t)c->chunk_rays, fine_row = (size_t)layer * R * c->cap_s2;
+  const void* src = what == 0   ? (const void*)(c->t_coarse + (size_t)layer * R * c->cap_n1)
+                    : what == 1 ? (const void*)(c->t_fine + fine_row)
+                    : what == 2 ? (const void*)(c->z_new + fine_row)
+                                : (const void*)(c->src_map + fine_row);
+  const size_t elem = what == 3 ? sizeof(uint8_t) : sizeof(float);
+  STNERF_CUDA(cudaMemcpyAsync(dst, src, (size_t)n_rays * S * elem, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return STNERF_OK;
 }
 
@@ -953,6 +964,36 @@ int stnerf_composite(const float* t, const float* rgb, const float* sigma, int64
                      float* depth, float* acc, float* w, void* stream) {
   if (!t || !rgb || !sigma || !color || !depth || !acc || S < 1) return STNERF_EINVAL;
   return launch_composite_simple(t, rgb, sigma, n, S, boarder, color, depth, acc, w, (cudaStream_t)stream);
+}
+
+int stnerf_composite_pass(const stnerf_scene* scene_host, int n_layers, int fine, const float* t, const float* raw,
+                          const uint8_t* mask, const float* u, uint64_t seed, int64_t n, int S, int n2, int pixel_layout,
+                          float* images, float* t_fine, float* z_new, uint8_t* src_map, void* stream) {
+  if (!scene_host || !t || !raw || n < 0 || n_layers < 1 || n_layers > STNERF_MAX_LAYERS) return STNERF_EINVAL;
+  if ((n_layers > 1 && !mask) || (pixel_layout != 0 && pixel_layout != 1) || (fine != 0 && fine != 1)) return STNERF_EINVAL;
+  if (fine ? (S < 1 || S > STNERF_MAX_S || n2 != 0) : (S < 3 || S > STNERF_MAX_N1 || n2 < 0 || S + n2 > STNERF_MAX_S))
+    return STNERF_EINVAL;
+  if (n2 > 0 ? !t_fine : (!images || t_fine)) return STNERF_EINVAL;
+  // STNERF_PASS_GENERIC=1: a coarse pass takes the shared-memory path whatever its sample counts (A/B of the two paths)
+  const char* e = getenv("STNERF_PASS_GENERIC");
+  const bool generic = e && e[0] == '1';
+  if ((z_new == nullptr) != (src_map == nullptr)) return STNERF_EINVAL;
+  // the origin map is one byte per fine depth and only the register-resident resampling writes it
+  if (z_new && (n2 == 0 || generic || !composite_pass_in_registers(S, n2, fine) || S + n2 > 256)) return STNERF_EINVAL;
+  DevScene d;
+  dev_scene_from(*scene_host, n_layers, d);
+  CompositeArgs a;
+  memset(&a, 0, sizeof(a));
+  a.t = t; a.t_layer_stride = n * S;
+  a.raw = raw; a.raw_layer_stride = n * S * 4;
+  a.mask = mask; a.mask_layer_stride = n;
+  a.u = u; a.u_layer_stride = n * n2;
+  a.t_fine = t_fine; a.tf_layer_stride = n * (S + n2);
+  a.z_new = z_new; a.zn_layer_stride = n * n2;
+  a.src_map = src_map; a.sm_layer_stride = n * (S + n2);
+  a.out = images; a.pixel_layout = pixel_layout; a.n_total = n; a.ray_base = 0; a.n = n;
+  a.S = S; a.n2 = n2; a.fine = fine; a.seed = seed; a.idmap = RayIdMap{0, 0, 0};
+  return launch_composite_pass(a, d, n_layers, (cudaStream_t)stream, generic);
 }
 
 int stnerf_sample_pdf(const float* t, const float* w, const float* u, int64_t n, int n1, int n2, float* z, float* t_fine,

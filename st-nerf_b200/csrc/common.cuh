@@ -201,7 +201,11 @@ struct CompositeArgs {
   uint64_t seed;
   RayIdMap idmap;
 };
-int launch_composite_pass(const CompositeArgs& a, const DevScene& scene, int n_layers, cudaStream_t st);
+// `force_generic`: run a coarse pass on the shared-memory path whatever its sample counts (stnerf_composite_pass: the register
+// path and the generic path are two implementations of one function).  The generic path writes no z_new / src_map.
+int launch_composite_pass(const CompositeArgs& a, const DevScene& scene, int n_layers, cudaStream_t st, bool force_generic = false);
+// the sample counts whose coarse pass composites and resamples in registers (and can write z_new / src_map)
+bool composite_pass_in_registers(int S, int n2, int fine);
 int launch_composite_simple(const float* t, const float* rgb, const float* sigma, long long n, int S, float boarder,
                             float* color, float* depth, float* acc, float* w, cudaStream_t st);
 int launch_composite_backward(const float* t, const float* rgb, const float* sigma, long long n, int S, float boarder,

@@ -36,9 +36,10 @@ __device__ __forceinline__ float warp_incl_add(float v, int lane) {
 }
 __device__ __forceinline__ float sigmoidf_ref(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// order-preserving map float -> uint32 (total order incl. negatives)
+// order-preserving map float -> uint32 (total order incl. negatives; -0.0 and +0.0 share a key, as they compare equal in the
+// reference's torch.sort and in the rank merge's <= / <)
 __device__ __forceinline__ uint32_t float_key(float f) {
-  const uint32_t u = __float_as_uint(f);
+  const uint32_t u = __float_as_uint(f + 0.0f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -462,10 +463,12 @@ static int launch_pass_t(const CompositeArgs& a, const DevScene& scene, int n_la
   return STNERF_OK;
 }
 
-int launch_composite_pass(const CompositeArgs& a, const DevScene& scene, int n_layers, cudaStream_t st) {
+bool composite_pass_in_registers(int S, int n2, int fine) { return !fine && S <= 128 && n2 <= 256; }
+
+int launch_composite_pass(const CompositeArgs& a, const DevScene& scene, int n_layers, cudaStream_t st, bool force_generic) {
   if (a.n <= 0) return STNERF_OK;
   if (a.S > STNERF_MAX_S || n_layers > STNERF_MAX_LAYERS) return STNERF_EINVAL;
-  const bool regs = !a.fine && a.S <= 128 && a.n2 <= 256;
+  const bool regs = composite_pass_in_registers(a.S, a.n2, a.fine) && !force_generic;
   const PassSmem L = pass_layout(n_layers, a.S, a.fine ? 0 : a.n2, regs);
   if (regs) {
     // coarse pass: register-resident per-layer composite + resampling, instantiated for the slot counts in use

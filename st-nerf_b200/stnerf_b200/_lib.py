@@ -70,6 +70,8 @@ _SIGNATURES = {
     "stnerf_intersect_sample": (C.c_int, [_P, C.c_int64, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
     "stnerf_composite": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P, _P, _P, _P]),
     "stnerf_sample_pdf": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int, C.c_int, _P, _P, _P]),
+    "stnerf_composite_pass": (C.c_int, [C.POINTER(Scene), C.c_int, C.c_int, _P, _P, _P, _P, C.c_uint64, C.c_int64, C.c_int, C.c_int,
+                                        C.c_int, _P, _P, _P, _P, _P]),
     "stnerf_positional_encoding": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
     "stnerf_spacenet": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P]),
     "stnerf_motionnet": (C.c_int, [_P, C.c_int, _P, C.c_int64, C.c_int, _P, _P]),

@@ -230,6 +230,17 @@ class NativeRenderer:
                                                  L.stream_ptr()), "stnerf_debug_read_depths")
         return out
 
+    def read_origin(self, layer: int, n_rays: int, n1: int, n2: int):
+        """z_new (n_rays, n2) and src_map (n_rays, n1+n2) uint8 of `layer` from the last chunk rendered: the new depths in
+        ascending order and where every fine depth came from.  Raises unless that render reused the coarse pass' flow."""
+        dev = torch.device("cuda", torch.cuda.current_device())
+        z = torch.empty((n_rays, n2), dtype=torch.float32, device=dev)
+        src = torch.empty((n_rays, n1 + n2), dtype=torch.uint8, device=dev)
+        for what, dst in ((2, z), (3, src)):
+            L.check(L.lib().stnerf_debug_read_depths(self._h, what, int(layer), L.ptr(dst), int(n_rays), int(dst.shape[1]),
+                                                     L.stream_ptr()), "stnerf_debug_read_depths")
+        return z, src
+
     def set_ray_ids(self, base: int = 0, width: int = 0, row_stride: int = 0):
         """Philox keys of the rays of subsequent render calls (see include/stnerf.h: stnerf_set_ray_ids)."""
         L.check(L.lib().stnerf_set_ray_ids(self._h, int(base), int(width), int(row_stride)), "stnerf_set_ray_ids")

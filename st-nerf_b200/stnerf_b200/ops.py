@@ -2,6 +2,8 @@
 entry point.  Inputs are CUDA fp32 tensors; outputs are fresh CUDA tensors.  No CPU fallback."""
 from __future__ import annotations
 
+import ctypes
+
 import torch
 
 from . import _lib as L
@@ -57,6 +59,41 @@ def sample_pdf(t, w, u, merge: bool = False):
     L.check(L.lib().stnerf_sample_pdf(L.ptr(t), L.ptr(w), L.ptr(u), N, n1, n2, L.ptr(z), L.ptr(tf), L.stream_ptr()),
             "stnerf_sample_pdf")
     return (z, tf) if merge else z
+
+
+def composite_pass(scene: "L.Scene", t, raw, mask, fine: bool = False, n2: int = 0, u=None, seed: int = 0,
+                   pixel_layout: int = 0, want_images: bool = True, want_origin: bool = False, t_fine=None):
+    """One compositing pass of the render path on explicit network outputs (stnerf_composite_pass): density masks, every hit
+    layer's own image, the depth-ordered merge and, in a coarse pass with n2 > 0, the resampling.
+    t (l,N,S), raw (l,N,S,4) = rgb logits + raw sigma, mask (l,N) uint8/bool, u (l,N,n2) or None = Philox(seed).
+    Returns a dict: images (l+1, 5N) (pixel_layout 0: rgb (N,3) | depth (N) | acc (N) per image; 1: (N,5) interleaved),
+    t_fine (l,N,S+n2) when n2 > 0 (`t_fine`: a caller's buffer to write into -- rows of missed layers are left untouched),
+    and with want_origin z_new (l,N,n2) and src_map (l,N,S+n2) uint8."""
+    t, raw = _f32(t), _f32(raw)
+    l, N, S = t.shape
+    assert tuple(raw.shape) == (l, N, S, 4), tuple(raw.shape)
+    mask = mask.to(device=t.device, dtype=torch.uint8).contiguous()
+    assert tuple(mask.shape) == (l, N), tuple(mask.shape)
+    if u is not None:
+        u = _f32(u)
+        assert tuple(u.shape) == (l, N, n2), tuple(u.shape)
+    out = {}
+    if want_images:
+        out["images"] = torch.empty((l + 1, 5 * N), dtype=torch.float32, device=t.device)
+    if n2 > 0:
+        if t_fine is None:
+            t_fine = torch.zeros((l, N, S + n2), dtype=torch.float32, device=t.device)
+        assert t_fine.is_cuda and t_fine.dtype == torch.float32 and t_fine.is_contiguous() and tuple(t_fine.shape) == (l, N, S + n2)
+        out["t_fine"] = t_fine
+    if want_origin:
+        out["z_new"] = torch.zeros((l, N, n2), dtype=torch.float32, device=t.device)
+        out["src_map"] = torch.zeros((l, N, S + n2), dtype=torch.uint8, device=t.device)
+    with torch.cuda.device(t.device):
+        L.check(L.lib().stnerf_composite_pass(ctypes.byref(scene), l, 1 if fine else 0, L.ptr(t), L.ptr(raw), L.ptr(mask), L.ptr(u),
+                                              int(seed) & (2 ** 64 - 1), N, S, int(n2), int(pixel_layout),
+                                              L.ptr(out.get("images")), L.ptr(out.get("t_fine")), L.ptr(out.get("z_new")),
+                                              L.ptr(out.get("src_map")), L.stream_ptr()), "stnerf_composite_pass")
+    return out
 
 
 def positional_encoding(x, n_freq: int):
