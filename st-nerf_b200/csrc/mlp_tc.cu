@@ -6,8 +6,12 @@
 //     (FuseCoarse, below).  Warpgroups 1 and 2 are the math warpgroups: warpgroup 1 + w owns rows 64 w .. 64 w + 63 of the tile,
 //     issues their MMAs (wgmma m64 x N x k16, N = 256 or 128, accumulators in registers) and runs their epilogues.  The two
 //     math warpgroups share nothing but the weight ring, so while one runs its epilogue the other keeps the tensor cores busy;
-//   * activations (A operand) live in shared memory as fp16 hi/lo pairs in the canonical 128B-swizzled K-major layout
-//     ([128 rows x 64 k] blocks); a layer's epilogue overwrites the rows its own MMAs have just finished reading;
+//   * activations (A operand) are fp16 hi/lo pairs.  The hi halves (and the whole encoding) live in shared memory in the
+//     canonical 128B-swizzled K-major layout ([128 rows x 64 k] blocks); a layer's epilogue overwrites the rows its own MMAs
+//     have just finished reading.  In the SpaceNet kernel the lo halves of the hidden activations stay in the math threads'
+//     registers, in the wgmma A-fragment layout the accumulator already has (epi_hidden), and Alo*Whi is the register-A form
+//     of wgmma; that frees 64 KB of shared memory for a 7-deep weight ring, and setmaxnreg moves registers from warpgroup 0
+//     to the math warpgroups to hold them;
 //   * weights (B operand) are pre-packed on the host into [N out-rows x 32 k] fp16 blocks that are already the 64B-swizzled
 //     shared-memory image -- per layer the hi and then the lo stage of every 32-k sub-chunk, in the layer's K order, each
 //     stored once -- and stream through a ring of stages with 1-D bulk async copies (cp.async.bulk + mbarrier complete_tx) from
@@ -44,6 +48,10 @@ constexpr int STAGE_BYTES = 16384;           // weight stage   [256 rows x 32 k]
 constexpr int NTHREADS = 384;                // warpgroup 0: producer + compositing warps; warpgroups 1, 2: math
 constexpr int MATH_WG0 = 1, N_MATH_WARPS = 8;
 constexpr int MAX_STAGE = 8;
+// registers per thread after setmaxnreg (SpaceNet kernel): warpgroup 0 (producer, compositing warps) and the math warpgroups;
+// 128 REGS_WG0 + 256 REGS_MATH must not exceed the 384 x 168 the launch allocates
+constexpr int REGS_WG0 = 56, REGS_MATH = 224;
+static_assert(128 * REGS_WG0 + 256 * REGS_MATH <= 384 * 168, "register file");
 constexpr int BAR_WFULL = 0, BAR_WEMPTY = 8, BAR_RAWFULL = 16, BAR_RAWEMPTY = 18;          // 20 barriers
 // misc region: barriers | per-row point info of the current tile | final rows for the compositing warps | their scratch
 constexpr int MISC_ROWS = 256;               // Pt[128]
@@ -92,6 +100,11 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 }
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// per-thread register budget of the whole warpgroup (sm_90a); every thread of the warpgroup executes the same one
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // named barrier of one math warpgroup (ids 1, 2; id 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
@@ -128,36 +141,35 @@ __device__ __forceinline__ void acc_fence(float (&d)[128]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// fp32 accumulator operands of an m64nNk16 wgmma: %0 .. %63 (N = 128), then %64 .. %127 (N = 256), and their constraints
+#define WGMMA_D_LO "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define WGMMA_D_HI "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define WGMMA_OPS_LO(d) \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+    "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+    "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+    "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+    "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+    "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define WGMMA_OPS_HI(d) \
+    "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), \
+    "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), \
+    "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), \
+    "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), \
+    "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), \
+    "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+    "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+    "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+
 // D[64 x 256] += A[64 x 16] * B[256 x 16]^T, both K-major in shared memory; fp16 in, fp32 accumulate in registers
 __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      "{" WGMMA_D_LO ", " WGMMA_D_HI "}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : WGMMA_OPS_LO(d), WGMMA_OPS_HI(d)
       : "l"(da), "l"(db), "r"(1));
 }
 // D[64 x 128] += A[64 x 16] * B[128 x 16]^T, both K-major in shared memory; fp16 in, fp32 accumulate in registers
@@ -165,26 +177,39 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[128], uint64_t da, uint64_
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      "{" WGMMA_D_LO "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : WGMMA_OPS_LO(d)
       : "l"(da), "l"(db), "r"(1));
+}
+// The same with A in registers: a[0..3] is this thread's fragment of the 64 x 16 A slice (f16x2 each: rows r, r + 8 at columns
+// c, c + 1, then the same rows at columns c + 8, c + 9, with r and c as in the accumulator fragment -- see epi_hidden).
+// wgmma reads the registers asynchronously: they must not change before the MMA has retired (wgmma.wait_group).
+__device__ __forceinline__ void wgmma_n256_rs(float (&d)[128], const uint32_t* a, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{" WGMMA_D_LO ", " WGMMA_D_HI "}, {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+      : WGMMA_OPS_LO(d), WGMMA_OPS_HI(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_n128_rs(float (&d)[128], const uint32_t* a, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{" WGMMA_D_LO "}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : WGMMA_OPS_LO(d)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
 }
 
 template <int N>
 __device__ __forceinline__ void wgmma_k16(float (&d)[128], uint64_t da, uint64_t db) {
   if (N == 256) wgmma_n256(d, da, db);
   else wgmma_n128(d, da, db);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_k16_rs(float (&d)[128], const uint32_t* a, uint64_t db) {
+  if (N == 256) wgmma_n256_rs(d, a, db);
+  else wgmma_n128_rs(d, a, db);
 }
 
 // {lo16 = fp16(a), hi16 = fp16(b)}, saturating to +-65504 (fp16 range guard of the split)
@@ -214,12 +239,13 @@ enum { NET_SPACE = 0, NET_MOTION = 1 };
 template <int NET> struct Sched;
 template <> struct Sched<NET_SPACE> {
   static constexpr int N_LAYERS = 8;
-  // shared memory: activations (4 hi + 4 lo blocks), encoding (hi, lo), a 3-deep ring of 16 KB weight stages, misc
-  static constexpr int act_base = 0, enc_base = 8 * ABLOCK;
-  static constexpr int LO_STRIDE = 4 * ABLOCK;          // ACT lo blocks follow the 4 hi blocks
+  // shared memory: activations (4 hi blocks), encoding (hi, lo), a 7-deep ring of 16 KB weight stages, misc.  The lo halves of
+  // the activations never reach shared memory: each math thread keeps its fragment of them in registers (lo_in_regs, epi_hidden)
+  static constexpr bool lo_in_regs = true;
+  static constexpr int act_base = 0, enc_base = 4 * ABLOCK;
   static constexpr int ENC_LO_STRIDE = ABLOCK;
-  static constexpr int n_stage = 3, stage_bytes = STAGE_BYTES;
-  static constexpr int ring_base = 10 * ABLOCK, misc_base = ring_base + n_stage * stage_bytes, smem_total = misc_base + MISC_TOTAL;
+  static constexpr int n_stage = 7, stage_bytes = STAGE_BYTES;
+  static constexpr int ring_base = 6 * ABLOCK, misc_base = ring_base + n_stage * stage_bytes, smem_total = misc_base + MISC_TOTAL;
   static_assert(smem_total <= 232448, "shared memory budget (227 KB per CTA)");
   __host__ __device__ static constexpr int n_out(int l) { return l == 7 ? 128 : 256; }
   __host__ __device__ static constexpr int act_chunks(int l) { return l == 0 ? 0 : 4; }
@@ -230,6 +256,7 @@ template <> struct Sched<NET_SPACE> {
 template <> struct Sched<NET_MOTION> {
   static constexpr int N_LAYERS = 5;
   // the encoding (read by layer 0 only) shares the activation blocks: layer 0's epilogue overwrites it after its MMAs retired
+  static constexpr bool lo_in_regs = false;
   static constexpr int act_base = 0, enc_base = 0;
   static constexpr int LO_STRIDE = 2 * ABLOCK;
   static constexpr int ENC_LO_STRIDE = 2 * ABLOCK;
@@ -584,9 +611,11 @@ __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float
 // MMAs of layer l for this warpgroup's 64 rows (A rows at byte offset a_row of every activation / encoding block), one weight
 // stage per step of WSched.  A stage is handed back (one arrival per math warp on w_empty) once the MMAs that read it have
 // retired: wgmma.wait_group 1 after the next stage's MMAs are issued keeps one stage of MMAs in flight.
+// S::lo_in_regs: the lo halves of the activation chunks are the register fragments alo (written by epi_hidden); the encoding
+// chunks keep both halves in shared memory.
 template <int NET, int N, bool LOFIRST>
-__device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uint32_t sbase, uint32_t a_row, uint32_t bars,
-                                          uint32_t& cnt, int lane) {
+__device__ __forceinline__ void mma_layer(float (&acc)[128], const uint32_t (&alo)[64], int l, bool sp, uint32_t sbase,
+                                          uint32_t a_row, uint32_t bars, uint32_t& cnt, int lane) {
   using S = Sched<NET>;
   using W = WSched<NET>;
   constexpr uint32_t NST = S::n_stage;
@@ -600,29 +629,49 @@ __device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uin
     __syncwarp();
     mbar_arrive_if(bars + 8u * (uint32_t)(BAR_WEMPTY + s), lane == 0);
   };
-  // hi / lo halves of A chunk ch (64 k): activation chunks 0..nact-1, then the encoding chunks
+  // hi / lo halves of A chunk ch (64 k): activation chunks 0..nact-1, then the encoding chunks.  z = the activation chunk whose
+  // lo half is in registers, or -1 (lo in shared memory)
   auto a_block = [&](int ch) {
-    uint32_t hi, lo;
+    uint32_t hi, lo = 0;
+    int z = -1;
     if (ch < nact) {
       hi = sbase + S::act_base + ch * ABLOCK + a_row;
-      lo = hi + S::LO_STRIDE;
+      if constexpr (S::lo_in_regs) z = ch;
+      else lo = hi + S::LO_STRIDE;
     } else {
       hi = sbase + S::enc_base + (ch - nact) * ABLOCK + a_row;
       lo = hi + S::ENC_LO_STRIDE;
     }
-    return make_uint2(hi, lo);
+    return make_int3((int)hi, (int)lo, z);
   };
-  W::template for_each_step<LOFIRST>(l, sp, a_block, [&](const uint2& a, auto st) {
-    const uint32_t hi = a.x + 64u * st.sub, lo = a.y + 64u * st.sub;
-    const uint32_t a0 = decltype(st)::a == A_LO ? lo : hi;
+  W::template for_each_step<LOFIRST>(l, sp, a_block, [&](const int3& a, auto st) {
+    const uint32_t hi = (uint32_t)a.x + 64u * st.sub, lo = (uint32_t)a.y + 64u * st.sub;
     const uint32_t s = cnt % NST, n = cnt / NST;
     mbar_wait(bars + 8u * (BAR_WFULL + s), n & 1);
     const uint32_t w = sbase + S::ring_base + s * S::stage_bytes;
+    // the two k16 MMAs of this stage with A = the lo half of the sub-chunk
+    auto mma_lo = [&]() {
+      if (S::lo_in_regs && a.z >= 0) {
+        // register fragments of 32-k sub-chunk q = 2 z + sub of the 256 activation columns: alo[8 q .. 8 q + 7].  The
+        // branches are warpgroup-uniform (z and sub come from the step loop); registers are indexed by constants only.
+        const int q = 2 * a.z + (int)st.sub;
 #pragma unroll
-    for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(a0 + ks * 32), desc_sw64(w + ks * 32));
-    if constexpr (decltype(st)::a == A_HI_LO) {
+        for (int i = 0; i < 8; ++i)
+          if (q == i) {
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(lo + ks * 32), desc_sw64(w + ks * 32));
+            for (int ks = 0; ks < 2; ++ks) wgmma_k16_rs<N>(acc, &alo[8 * i + 4 * ks], desc_sw64(w + ks * 32));
+          }
+      } else {
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(lo + ks * 32), desc_sw64(w + ks * 32));
+      }
+    };
+    if constexpr (decltype(st)::a == A_LO) {
+      mma_lo();
+    } else {
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) wgmma_k16<N>(acc, desc_sw128(hi + ks * 32), desc_sw64(w + ks * 32));
+      if constexpr (decltype(st)::a == A_HI_LO) mma_lo();
     }
     wgmma_commit();
     wgmma_wait<1>();
@@ -637,9 +686,13 @@ __device__ __forceinline__ void mma_layer(float (&acc)[128], int l, bool sp, uin
 
 // Hidden-layer epilogue from the accumulator fragment: bias, ReLU, fp16 hi (+ lo) split into the activation blocks (rows r0 and
 // r0 + 8, columns 8 j + cq, +1 for j < N / 8); SIGMA: the density head's partial dot products of the two rows.
+// S::lo_in_regs: lo goes to alo[2 j] (row r0) and alo[2 j + 1] (row r0 + 8) instead.  Column groups 2 k and 2 k + 1 of the
+// accumulator fragment are exactly the register A fragment of k16-slice k of the next layer, so alo[4 k .. 4 k + 3] is that
+// slice's A operand as it is (wgmma_n256_rs).
 template <int NET, int N, bool SIGMA>
 __device__ __forceinline__ void epi_hidden(const float (&acc)[128], const float* __restrict__ bias, const float* __restrict__ wsig,
-                                           uint8_t* smem, int r0, int cq, bool lo_too, float& sig0, float& sig1) {
+                                           uint8_t* smem, int r0, int cq, bool lo_too, float& sig0, float& sig1,
+                                           uint32_t (&alo)[64]) {
   using S = Sched<NET>;
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
@@ -657,10 +710,16 @@ __device__ __forceinline__ void epi_hidden(const float (&acc)[128], const float*
     const uint32_t h0 = pack_f16x2(v00, v01), h1 = pack_f16x2(v10, v11);
     *reinterpret_cast<uint32_t*>(blk + o0) = h0;
     *reinterpret_cast<uint32_t*>(blk + o1) = h1;
-    if (lo_too) {
-      const float2 f0 = unpack_f16x2(h0), f1 = unpack_f16x2(h1);
-      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o0) = pack_f16x2(v00 - f0.x, v01 - f0.y);
-      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o1) = pack_f16x2(v10 - f1.x, v11 - f1.y);
+    const float2 f0 = unpack_f16x2(h0), f1 = unpack_f16x2(h1);
+    const uint32_t l0 = pack_f16x2(v00 - f0.x, v01 - f0.y), l1 = pack_f16x2(v10 - f1.x, v11 - f1.y);
+    if constexpr (S::lo_in_regs) {
+      // written whether the next layer reads them or not: a conditional write would keep the previous layer's fragments
+      // alive through the epilogue next to the accumulator
+      alo[2 * j] = l0;
+      alo[2 * j + 1] = l1;
+    } else if (lo_too) {
+      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o0) = l0;
+      *reinterpret_cast<uint32_t*>(blk + S::LO_STRIDE + o1) = l1;
     }
   }
 }
@@ -707,33 +766,40 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_consta
   }
   __syncthreads();
 
-  if (warp == 0) {
-    // =============================== weight producer: the whole warp runs the loop, one elected lane issues ===============================
-    using W = WSched<NET>;
-    uint32_t cnt = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const uint8_t* layer = P.wstream;
-      for (int l = 0; l < S::N_LAYERS; ++l) {
-        W::template for_each_step<LOFIRST>(l, split(l), [](int) { return 0; }, [&](int, auto st) {
-          const uint32_t s = cnt % NST, n = cnt / NST;
-          mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
-          load_stage_elect(sbase + S::ring_base + s * S::stage_bytes, layer + st.offset, W::stage_bytes(l), BAR(BAR_WFULL + s));
-          ++cnt;
-        });
-        layer += W::layer_bytes(l);
+  // SpaceNet (S::lo_in_regs): the math threads hold the accumulator (128 registers) and the lo activation fragments (64), so
+  // warpgroup 0 hands registers over to them.  Each role's setmaxnreg sits inside its branch, where ptxas can tell which
+  // budget the code after it runs under.
+  if (wgi < MATH_WG0) {
+    if constexpr (S::lo_in_regs) setmaxnreg_dec<REGS_WG0>();
+    if (warp == 0) {
+      // =============================== weight producer: the whole warp runs the loop, one elected lane issues ===============================
+      using W = WSched<NET>;
+      uint32_t cnt = 0;
+      for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const uint8_t* layer = P.wstream;
+        for (int l = 0; l < S::N_LAYERS; ++l) {
+          W::template for_each_step<LOFIRST>(l, split(l), [](int) { return 0; }, [&](int, auto st) {
+            const uint32_t s = cnt % NST, n = cnt / NST;
+            mbar_wait(BAR(BAR_WEMPTY + s), (n & 1) ^ 1);
+            load_stage_elect(sbase + S::ring_base + s * S::stage_bytes, layer + st.offset, W::stage_bytes(l), BAR(BAR_WFULL + s));
+            ++cnt;
+          });
+          layer += W::layer_bytes(l);
+        }
+      }
+    } else if (NET == NET_SPACE && (warp == 2 || warp == 3)) {
+      // =============================== compositing warps (coarse-pass fusion) ===============================
+      if (P.fuse.on) {
+        const int j = warp - 2;
+        float* cdf = reinterpret_cast<float*>(smem + S::misc_base + MISC_CDF) + j * 64;
+        if (P.fuse.n2 <= 128)
+          fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
+        else
+          fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
       }
     }
-  } else if (NET == NET_SPACE && (warp == 2 || warp == 3)) {
-    // =============================== compositing warps (coarse-pass fusion) ===============================
-    if (P.fuse.on) {
-      const int j = warp - 2;
-      float* cdf = reinterpret_cast<float*>(smem + S::misc_base + MISC_CDF) + j * 64;
-      if (P.fuse.n2 <= 128)
-        fused_composite_loop<4>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
-      else
-        fused_composite_loop<8>(P, s_part, cdf, BAR(BAR_RAWFULL + j), BAR(BAR_RAWEMPTY + j), n_tiles, j, lane);
-    }
-  } else if (wgi >= MATH_WG0) {
+  } else {
+    if constexpr (S::lo_in_regs) setmaxnreg_inc<REGS_MATH>();
     // =============================== math warpgroups: encoding, MMAs, epilogues ===============================
     const int wg = wgi - MATH_WG0;                    // 0, 1: rows 64 wg .. 64 wg + 63 of every tile
     const int wt = tid & 127;
@@ -746,6 +812,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_consta
     const bool fused = (NET == NET_SPACE) && P.fuse.on;
     uint32_t cnt = 0, tile_no = 0;
     float acc[128];
+    uint32_t alo[64];                                  // S::lo_in_regs: lo activations of the last hidden layer (epi_hidden)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) alo[i] = 0u;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tile_no) {
       // the previous tile's MMAs have retired in every warp of the warpgroup and its rows are written out: its blocks are free
       wg_bar_sync(wg);
@@ -771,16 +840,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp_tc_kernel(const __grid_consta
         wg_bar_sync(wg);
         const bool last = (l == S::N_LAYERS - 1);
         if (!last) {
-          mma_layer<NET, (NET == NET_SPACE ? 256 : 128), LOFIRST>(acc, l, split(l), sbase, a_row, bars, cnt, lane);
+          mma_layer<NET, (NET == NET_SPACE ? 256 : 128), LOFIRST>(acc, alo, l, split(l), sbase, a_row, bars, cnt, lane);
           if (NET == NET_SPACE && l == 6)
-            epi_hidden<NET, 256, true>(acc, bias_all + l * 256, P.aux + AUX_WSIG, smem, r0, cq, split(l + 1), sig0, sig1);
+            epi_hidden<NET, 256, true>(acc, bias_all + l * 256, P.aux + AUX_WSIG, smem, r0, cq, split(l + 1), sig0, sig1, alo);
           else
-            epi_hidden<NET, (NET == NET_SPACE ? 256 : 128), false>(acc, bias_all + l * 256, nullptr, smem, r0, cq, split(l + 1), sig0, sig1);
+            epi_hidden<NET, (NET == NET_SPACE ? 256 : 128), false>(acc, bias_all + l * 256, nullptr, smem, r0, cq, split(l + 1), sig0,
+                                                                  sig1, alo);
           continue;
         }
         // last layer: 128 features -> 3-wide head in fp32 (rgb_net.3 / motion_net.10).
         // SpaceNet: the bias is the per-ray vector of head_bias_kernel (dir/time part of rgb_net.1 + b1).
-        mma_layer<NET, 128, LOFIRST>(acc, l, split(l), sbase, a_row, bars, cnt, lane);
+        mma_layer<NET, 128, LOFIRST>(acc, alo, l, split(l), sbase, a_row, bars, cnt, lane);
         const Pt p0 = s_rows[r0], p1 = s_rows[r0 + 8];
         const float* b0 = (NET == NET_SPACE) ? (P.cbuf + (size_t)p0.cidx * 128) : bias_all + l * 256;
         const float* b1 = (NET == NET_SPACE) ? (P.cbuf + (size_t)p1.cidx * 128) : bias_all + l * 256;
