@@ -223,7 +223,17 @@ int stnerf_spacenet(stnerf_handle h, int layer, int fine, const float* pos, cons
 int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
                      void* stream);
 
-/* ---- training: differentiable SpaceNet / MotionNet in fp32 on CUDA cores (no context) ------------------------------------
+/* ---- training: differentiable SpaceNet / MotionNet (no context) ------------------------------------------------------------
+ * Training precision of the _prec entry points below; the entry points without _prec are STNERF_TRAIN_FP32.               */
+enum {
+  STNERF_TRAIN_FP32 = 0,       /* fp32 FFMA on CUDA cores; the forward is bit-identical to STNERF_PREC_FP32_SIMT            */
+  STNERF_TRAIN_TC_3XTF32 = 1   /* every GEMM of a layer with 128 or more outputs (SpaceNet trunk + rgb_net.1, MotionNet
+                                  motion_net.0-.8: forward, input deltas, weight gradients) on wgmma with 3xTF32 products
+                                  (Alo*Bhi + Ahi*Blo + Ahi*Bhi, tf32 hi/lo split, fp32 accumulate, promoted into an fp32 total
+                                  every 32 k): ~22 significant bits per product with fp32's exponent range.  The 1- and 3-wide
+                                  heads stay fp32.  Its forward is NOT bit-identical to any STNERF_PREC_* render mode.       */
+};
+/* ---- fp32 on CUDA cores unless a _prec entry point is given STNERF_TRAIN_TC_3XTF32 ---------------------------------------
  * `weights` is a DEVICE blob in the stnerf_load_* order above (state_dict order, nn.Linear (out,in) row-major), read in place;
  * `d_weights` receives the gradient of every tensor in the same order and size (464260 / 466948 / 77315 floats).
  * A training forward fills `saved` (stnerf_train_saved_floats floats) with what the backward of the same points needs: the
@@ -250,6 +260,19 @@ int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int6
 /* Gradient of motion_net.py:34-71 for d_flow (P,3): d_weights only (xyzt is detached, layered_rfrender.py:314-315). */
 int stnerf_motionnet_backward(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
                               void* scratch, size_t scratch_bytes, void* stream);
+/* The same four calls in a training precision (STNERF_TRAIN_*; the `saved` layout is the same for both).  A backward must
+ * run in the precision of the forward that filled `saved`.  An unknown precision, or a scratch buffer smaller than
+ * stnerf_train_scratch_bytes_prec reports, returns STNERF_EINVAL (stnerf_train_scratch_bytes_prec then returns 0). */
+size_t stnerf_train_scratch_bytes_prec(int kind, int use_time, int64_t P, int precision);
+int stnerf_spacenet_train_forward_prec(const float* weights, int use_time, const float* pos, const float* dirs, const float* times,
+                                       int64_t P, float* rgb, float* sigma, float* saved, int precision, void* stream);
+int stnerf_spacenet_backward_prec(const float* weights, int use_time, int64_t P, const float* saved, const float* d_rgb,
+                                  const float* d_sigma, float* d_weights, float* d_pos, void* scratch, size_t scratch_bytes,
+                                  int precision, void* stream);
+int stnerf_motionnet_train_forward_prec(const float* weights, const float* xyzt, int64_t P, int lerp_mode, float* flow,
+                                        float* saved, void* scratch, size_t scratch_bytes, int precision, void* stream);
+int stnerf_motionnet_backward_prec(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
+                                   void* scratch, size_t scratch_bytes, int precision, void* stream);
 /* Gradient of layers/render_layer.py:8-58 (gen_weight + VolumeRenderer.forward) for stnerf_composite's outputs.
  * d_color (n,3), d_depth (n), d_acc (n), d_w (n,S): any may be NULL (zero).  -> d_rgb (n,S,3), d_sigma (n,S).
  * t gets no gradient (the reference detaches every depth it composites, layered_rfrender.py:314,461).

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Forward + backward of one SpaceNet and one MotionNet on the native fp32 training kernels (stnerf_b200.nets), against the
-same step through torch fp32 autograd (cuBLAS, TF32 off) on the same GPU.
+"""Forward + backward of one SpaceNet and one MotionNet on the native training kernels (stnerf_b200.nets), against the
+same step through torch fp32 autograd (cuBLAS, TF32 off) on the same GPU, and -- for context only -- torch with TF32 on
+(arm "torch_1xtf32": one tf32 product per term, less accurate than the native tf32x3 precision).
 
-    python scripts/bench_train_nets.py [--log2p 16 17 18 19 20] [--warmup 3] [--iters 10]
+    python scripts/bench_train_nets.py [--log2p 16 17 18 19 20] [--warmup 3] [--iters 10] [--train-precision fp32|tf32x3]
 
 Per network and batch size P it prints ms per step, points/s and algorithmic FLOP/s, counted from the shapes:
   MACs per point = forward (every Linear: in x out)
@@ -92,16 +93,18 @@ def main():
     ap.add_argument("--log2p", type=int, nargs="+", default=[16, 17, 18, 19, 20])
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--train-precision", choices=["fp32", "tf32x3"], default="fp32", help="precision of the native arm")
     a = ap.parse_args()
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
     dev = torch.device("cuda")
     card, watts = torch.cuda.get_device_name(dev), power_limit()
-    print("# %s, power limit %s W; fp32 forward + backward per step" % (card, "%.0f" % watts if watts else "unknown"))
-    print("%-6s %8s %-7s %10s %14s %10s" % ("net", "P", "arm", "ms/step", "points/s", "TFLOP/s"))
+    print("# %s, power limit %s W; forward + backward per step, native arm in %s" % (card, "%.0f" % watts if watts else "unknown",
+                                                                                  a.train_precision))
+    print("%-6s %8s %-12s %10s %14s %10s" % ("net", "P", "arm", "ms/step", "points/s", "TFLOP/s"))
     torch.manual_seed(0)
-    sn = nets.SpaceNet(use_time=True).to(dev)
-    mn = nets.MotionNet(c_input=4, input_time=True).to(dev)
+    sn = nets.SpaceNet(use_time=True, train_precision=a.train_precision).to(dev)
+    mn = nets.MotionNet(c_input=4, input_time=True, train_precision=a.train_precision).to(dev)
     rows = []
     for lp in a.log2p:
         P = 1 << lp
@@ -126,18 +129,20 @@ def main():
         def motion_torch():
             (torch_motion(mn, xyzt) * r_flow).sum().backward()
 
-        for net, arms in (("space", (("native", space_native), ("torch", space_torch))),
-                          ("motion", (("native", motion_native), ("torch", motion_torch)))):
+        for net, arms in (("space", (("native", space_native), ("torch", space_torch), ("torch_1xtf32", space_torch))),
+                          ("motion", (("native", motion_native), ("torch", motion_torch), ("torch_1xtf32", motion_torch)))):
             for arm, step in arms:
+                torch.backends.cuda.matmul.allow_tf32 = arm == "torch_1xtf32"
                 ms = time_ms(step, a.warmup, a.iters)
                 tflops = 2.0 * macs(net) * P / (ms * 1e-3) / 1e12
-                print("%-6s %8d %-7s %10.3f %14.4g %10.2f" % (net, P, arm, ms, P / (ms * 1e-3), tflops))
+                print("%-6s %8d %-12s %10.3f %14.4g %10.2f" % (net, P, arm, ms, P / (ms * 1e-3), tflops))
                 rows.append({"net": net, "P": P, "arm": arm, "ms": ms, "points_per_s": P / (ms * 1e-3), "tflops": tflops})
         del pos, rays, tm, xyzt, r_rgb, r_sig, r_flow
         sn.zero_grad(set_to_none=True)
         mn.zero_grad(set_to_none=True)
         torch.cuda.empty_cache()
-    print(json.dumps({"card": card, "power_limit_w": watts, "rows": rows}))
+    torch.backends.cuda.matmul.allow_tf32 = False
+    print(json.dumps({"card": card, "power_limit_w": watts, "train_precision": a.train_precision, "rows": rows}))
 
 
 if __name__ == "__main__":

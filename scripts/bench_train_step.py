@@ -35,8 +35,8 @@ from tests_support import make_cfg  # noqa: E402
 N_RAYS, N1, N2, LAYERS = 2000, 90, 30, 2
 MASK_SCALAR = 100000.0
 LR = 4e-4
-# the kernels of csrc/mlp_train.cu (SpaceNet / MotionNet training forward and backward)
-NETWORK_KERNELS = ("gemm_kernel", "reduce_partials_kernel", "rowsum_kernel", "spacenet_encode_kernel", "motionnet_encode_kernel",
+# the kernels of csrc/mlp_train.cu and mlp_train_tc.cu (SpaceNet / MotionNet training forward and backward)
+NETWORK_KERNELS = ("gemm_kernel", "tc_gemm_kernel", "reduce_partials_kernel", "rowsum_kernel", "spacenet_encode_kernel", "motionnet_encode_kernel",
                    "spacenet_dpos_kernel")
 
 
@@ -129,16 +129,18 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--iters", type=int, default=10)
+    ap.add_argument("--train-precision", choices=["fp32", "tf32x3"], default="fp32", help="precision of the native networks")
     args = ap.parse_args()
     torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda", 0)
     card, watts = torch.cuda.get_device_name(dev), power_limit()
-    print("# %s, power limit %s W; training step, %d rays, %d performers, %d + %d samples"
-          % (card, "%.0f" % watts if watts else "unknown", N_RAYS, LAYERS, N1, N2))
+    print("# %s, power limit %s W; training step, %d rays, %d performers, %d + %d samples, native networks in %s"
+          % (card, "%.0f" % watts if watts else "unknown", N_RAYS, LAYERS, N1, N2, args.train_precision))
     import modeling
     case = dict(C.CASES["tkd_train_7col_mixed"], n_rays=N_RAYS, ray_seed=31, n1=N1, n2=N2)
     cfg = make_cfg(LAYERS, N1, N2, True, "fp32")
     cfg.MODEL.B200_TRAINABLE = True
+    cfg.MODEL.B200_TRAIN_PRECISION = args.train_precision
     model = modeling.build_layered_model(cfg, 0, None, None)
     model.load_state_dict(O.synthetic_state_dict(LAYERS, True, seed=3))
     bkgd, frames = C.boxes_for(case)
@@ -172,13 +174,15 @@ def main():
             opt.step()
         return run
 
-    def torch_step(only_coarse):
+    def torch_step(only_coarse, tf32=False):
         def run():
+            torch.backends.cuda.matmul.allow_tf32 = tf32
             ref_opt.zero_grad()
             out = torch_forward(ref_p, rays, t_c, mask, u, only_coarse, 0.0)
             loss = trainer_loss(out, rays, labels, target, only_coarse)
             loss.backward()
             ref_opt.step()
+            torch.backends.cuda.matmul.allow_tf32 = False
         return run
 
     def time_ms(fn):
@@ -195,7 +199,7 @@ def main():
 
     rows = []
     for stage, only_coarse in (("fine", False), ("coarse", True)):
-        times = {"native": [], "torch": []}
+        times = {"native": [], "torch": [], "torch_1xtf32": []}
         for _ in range(2):                                       # alternated
             torch.cuda.reset_peak_memory_stats(dev)
             times["native"].append(time_ms(native_step(only_coarse)))
@@ -203,7 +207,9 @@ def main():
             torch.cuda.reset_peak_memory_stats(dev)
             times["torch"].append(time_ms(torch_step(only_coarse)))
             peak_torch = torch.cuda.max_memory_allocated(dev)
-        nat_ms, ref_ms = min(times["native"]), min(times["torch"])
+            # context only: torch with TF32 matmuls (one tf32 product per term, less accurate than tf32x3)
+            times["torch_1xtf32"].append(time_ms(torch_step(only_coarse, tf32=True)))
+        nat_ms, ref_ms, tf32_ms = min(times["native"]), min(times["torch"]), min(times["torch_1xtf32"])
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             native_step(only_coarse)()
             torch.cuda.synchronize()
@@ -213,15 +219,17 @@ def main():
             tot_us += us
             if any(k in e.key for k in NETWORK_KERNELS):
                 net_us += us
-        row = dict(stage=stage, native_ms=round(nat_ms, 3), torch_ms=round(ref_ms, 3),
+        row = dict(stage=stage, train_precision=args.train_precision, native_ms=round(nat_ms, 3), torch_ms=round(ref_ms, 3),
+                   torch_1xtf32_ms=round(tf32_ms, 3),
                    native_rays_per_s=round(N_RAYS / nat_ms * 1e3), torch_rays_per_s=round(N_RAYS / ref_ms * 1e3),
                    network_share=round(net_us / tot_us, 3) if tot_us else None,
                    peak_mem_native_gb=round(peak_native / 2 ** 30, 2), peak_mem_torch_gb=round(peak_torch / 2 ** 30, 2),
                    hits=[int(x) for x in mask.sum(1)])
         rows.append(row)
-        print("%-6s native %.2f ms (%.0f rays/s), torch %.2f ms (%.0f rays/s); networks %.0f %% of native device time; "
-              "peak %.2f / %.2f GB" % (stage, nat_ms, row["native_rays_per_s"], ref_ms, row["torch_rays_per_s"],
-                                       100 * (row["network_share"] or 0), row["peak_mem_native_gb"], row["peak_mem_torch_gb"]))
+        print("%-6s native %.2f ms (%.0f rays/s), torch %.2f ms (%.0f rays/s), torch 1xTF32 %.2f ms; networks %.0f %% of native "
+              "device time; peak %.2f / %.2f GB" % (stage, nat_ms, row["native_rays_per_s"], ref_ms, row["torch_rays_per_s"], tf32_ms,
+                                                    100 * (row["network_share"] or 0), row["peak_mem_native_gb"],
+                                                    row["peak_mem_torch_gb"]))
         if stage == "fine":
             print("# kernels of one native step:")
             for e in sorted(prof.key_averages(), key=lambda e: -getattr(e, "device_time_total", 0))[:12]:

@@ -1051,7 +1051,9 @@ extern "C" int stnerf_motionnet(stnerf_handle c, int layer, const float* xyzt, i
   return run_motionnet(c, s, net, c->any_frac, lerp_mode, nullptr, flow, st);
 }
 
-// ---- training: fp32 forward with saved activations, and the backward (mlp_train.cu) ----------------------------------------
+// ---- training: forward with saved activations, and the backward (mlp_train.cu, mlp_train_tc.cu) -----------------------------
+static bool train_prec_ok(int prec) { return prec == STNERF_TRAIN_FP32 || prec == STNERF_TRAIN_TC_3XTF32; }
+
 extern "C" {
 
 size_t stnerf_train_saved_floats(int kind, int use_time, int64_t P) {
@@ -1059,38 +1061,57 @@ size_t stnerf_train_saved_floats(int kind, int use_time, int64_t P) {
   return train_saved_floats(kind, use_time != 0) * (size_t)P;
 }
 
+size_t stnerf_train_scratch_bytes_prec(int kind, int use_time, int64_t P, int precision) {
+  if ((kind != 0 && kind != 1) || P < 0 || !train_prec_ok(precision)) return 0;
+  return train_scratch_bytes(kind, use_time != 0, P);     // both precisions chunk the weight-gradient sums alike
+}
+
 size_t stnerf_train_scratch_bytes(int kind, int use_time, int64_t P) {
-  if ((kind != 0 && kind != 1) || P < 0) return 0;
-  return train_scratch_bytes(kind, use_time != 0, P);
+  return stnerf_train_scratch_bytes_prec(kind, use_time, P, STNERF_TRAIN_FP32);
+}
+
+int stnerf_spacenet_train_forward_prec(const float* weights, int use_time, const float* pos, const float* dirs, const float* times,
+                                       int64_t P, float* rgb, float* sigma, float* saved, int precision, void* stream) {
+  if (P < 0 || !train_prec_ok(precision)) return STNERF_EINVAL;
+  if (P == 0) return STNERF_OK;
+  if (!weights || !pos || !dirs || !rgb || !sigma || !saved || (use_time && !times)) return STNERF_EINVAL;
+  return launch_spacenet_train_forward(weights, use_time != 0, pos, dirs, times, P, rgb, sigma, saved, (cudaStream_t)stream,
+                                       precision);
 }
 
 int stnerf_spacenet_train_forward(const float* weights, int use_time, const float* pos, const float* dirs, const float* times,
                                   int64_t P, float* rgb, float* sigma, float* saved, void* stream) {
-  if (P < 0) return STNERF_EINVAL;
-  if (P == 0) return STNERF_OK;
-  if (!weights || !pos || !dirs || !rgb || !sigma || !saved || (use_time && !times)) return STNERF_EINVAL;
-  return launch_spacenet_train_forward(weights, use_time != 0, pos, dirs, times, P, rgb, sigma, saved, (cudaStream_t)stream);
+  return stnerf_spacenet_train_forward_prec(weights, use_time, pos, dirs, times, P, rgb, sigma, saved, STNERF_TRAIN_FP32, stream);
 }
 
-int stnerf_spacenet_backward(const float* weights, int use_time, int64_t P, const float* saved, const float* d_rgb,
-                             const float* d_sigma, float* d_weights, float* d_pos, void* scratch, size_t scratch_bytes,
-                             void* stream) {
-  if (P < 0 || !d_weights) return STNERF_EINVAL;
+int stnerf_spacenet_backward_prec(const float* weights, int use_time, int64_t P, const float* saved, const float* d_rgb,
+                                  const float* d_sigma, float* d_weights, float* d_pos, void* scratch, size_t scratch_bytes,
+                                  int precision, void* stream) {
+  if (P < 0 || !d_weights || !train_prec_ok(precision)) return STNERF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   if (P == 0) {                        // an empty batch contributes nothing to the gradient
     STNERF_CUDA(cudaMemsetAsync(d_weights, 0, (use_time ? SPACENET_FLOATS_TIME : SPACENET_FLOATS_NOTIME) * sizeof(float), st));
     return STNERF_OK;
   }
-  if (!weights || !saved || !d_rgb || !d_sigma || !scratch || scratch_bytes < train_scratch_bytes(0, use_time != 0, P))
+  if (!weights || !saved || !d_rgb || !d_sigma || !scratch ||
+      scratch_bytes < stnerf_train_scratch_bytes_prec(0, use_time, P, precision))
     return STNERF_EINVAL;
-  return launch_spacenet_backward(weights, use_time != 0, P, saved, d_rgb, d_sigma, d_weights, d_pos, scratch, st);
+  return launch_spacenet_backward(weights, use_time != 0, P, saved, d_rgb, d_sigma, d_weights, d_pos, scratch, st, precision);
 }
 
-int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int64_t P, int lerp_mode, float* flow, float* saved,
-                                   void* scratch, size_t scratch_bytes, void* stream) {
-  if (P < 0 || lerp_mode < -1 || lerp_mode > 1) return STNERF_EINVAL;
+int stnerf_spacenet_backward(const float* weights, int use_time, int64_t P, const float* saved, const float* d_rgb,
+                             const float* d_sigma, float* d_weights, float* d_pos, void* scratch, size_t scratch_bytes,
+                             void* stream) {
+  return stnerf_spacenet_backward_prec(weights, use_time, P, saved, d_rgb, d_sigma, d_weights, d_pos, scratch, scratch_bytes,
+                                       STNERF_TRAIN_FP32, stream);
+}
+
+int stnerf_motionnet_train_forward_prec(const float* weights, const float* xyzt, int64_t P, int lerp_mode, float* flow,
+                                        float* saved, void* scratch, size_t scratch_bytes, int precision, void* stream) {
+  if (P < 0 || lerp_mode < -1 || lerp_mode > 1 || !train_prec_ok(precision)) return STNERF_EINVAL;
   if (P == 0) return STNERF_OK;
-  if (!weights || !xyzt || !flow || !saved || !scratch || scratch_bytes < train_scratch_bytes(1, 0, P)) return STNERF_EINVAL;
+  if (!weights || !xyzt || !flow || !saved || !scratch || scratch_bytes < stnerf_train_scratch_bytes_prec(1, 0, P, precision))
+    return STNERF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   int* flag = (int*)scratch;
   if (lerp_mode < 0) {
@@ -1098,19 +1119,31 @@ int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int6
     any_fraction_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(xyzt, P, flag);
     STNERF_LAUNCH_CHECK();
   }
-  return launch_motionnet_train_forward(weights, xyzt, P, flag, lerp_mode, flow, saved, st);
+  return launch_motionnet_train_forward(weights, xyzt, P, flag, lerp_mode, flow, saved, st, precision);
 }
 
-int stnerf_motionnet_backward(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
-                              void* scratch, size_t scratch_bytes, void* stream) {
-  if (P < 0 || !d_weights) return STNERF_EINVAL;
+int stnerf_motionnet_train_forward(const float* weights, const float* xyzt, int64_t P, int lerp_mode, float* flow, float* saved,
+                                   void* scratch, size_t scratch_bytes, void* stream) {
+  return stnerf_motionnet_train_forward_prec(weights, xyzt, P, lerp_mode, flow, saved, scratch, scratch_bytes, STNERF_TRAIN_FP32,
+                                             stream);
+}
+
+int stnerf_motionnet_backward_prec(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
+                                   void* scratch, size_t scratch_bytes, int precision, void* stream) {
+  if (P < 0 || !d_weights || !train_prec_ok(precision)) return STNERF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   if (P == 0) {
     STNERF_CUDA(cudaMemsetAsync(d_weights, 0, MOTIONNET_FLOATS * sizeof(float), st));
     return STNERF_OK;
   }
-  if (!weights || !saved || !d_flow || !scratch || scratch_bytes < train_scratch_bytes(1, 0, P)) return STNERF_EINVAL;
-  return launch_motionnet_backward(weights, P, saved, d_flow, d_weights, scratch, st);
+  if (!weights || !saved || !d_flow || !scratch || scratch_bytes < stnerf_train_scratch_bytes_prec(1, 0, P, precision))
+    return STNERF_EINVAL;
+  return launch_motionnet_backward(weights, P, saved, d_flow, d_weights, scratch, st, precision);
+}
+
+int stnerf_motionnet_backward(const float* weights, int64_t P, const float* saved, const float* d_flow, float* d_weights,
+                              void* scratch, size_t scratch_bytes, void* stream) {
+  return stnerf_motionnet_backward_prec(weights, P, saved, d_flow, d_weights, scratch, scratch_bytes, STNERF_TRAIN_FP32, stream);
 }
 
 int stnerf_composite_backward(const float* t, const float* rgb, const float* sigma, int64_t n, int S, float boarder,

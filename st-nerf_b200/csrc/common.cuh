@@ -221,17 +221,18 @@ int launch_motionnet_simt(const PointSrc& src, const MotionNetW& w, const int* l
                           float* xyz_out, float* flow_out, int num_sms, cudaStream_t st);
 size_t simt_smem_bytes();
 
-// mlp_train.cu (kind 0 = SpaceNet, 1 = MotionNet; W / dW = stnerf_load_* blobs)
+// mlp_train.cu (kind 0 = SpaceNet, 1 = MotionNet; W / dW = stnerf_load_* blobs), with mlp_train_tc.cu
 size_t train_saved_floats(int kind, int use_time);
 size_t train_scratch_bytes(int kind, int use_time, long long P);
+// prec: STNERF_TRAIN_FP32 or STNERF_TRAIN_TC_3XTF32 (validated by the caller)
 int launch_spacenet_train_forward(const float* W, int use_time, const float* pos, const float* dirs, const float* times,
-                                  long long P, float* rgb, float* sigma, float* saved, cudaStream_t st);
+                                  long long P, float* rgb, float* sigma, float* saved, cudaStream_t st, int prec);
 int launch_spacenet_backward(const float* W, int use_time, long long P, const float* saved, const float* d_rgb,
-                             const float* d_sigma, float* dW, float* d_pos, void* scratch, cudaStream_t st);
+                             const float* d_sigma, float* dW, float* d_pos, void* scratch, cudaStream_t st, int prec);
 int launch_motionnet_train_forward(const float* W, const float* xyzt, long long P, const int* lerp_flag, int lerp_force,
-                                   float* flow, float* saved, cudaStream_t st);
+                                   float* flow, float* saved, cudaStream_t st, int prec);
 int launch_motionnet_backward(const float* W, long long P, const float* saved, const float* d_flow, float* dW, void* scratch,
-                              cudaStream_t st);
+                              cudaStream_t st, int prec);
 
 // train_march.cu (the per-sample work of a training step around the networks)
 size_t train_hits_scratch_ints(long long n, int n_layers);

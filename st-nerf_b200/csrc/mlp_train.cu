@@ -18,9 +18,13 @@
 // dense_layer in mlp_simt.cu, and the encodings use the same sincosf arguments: the training forward is bit-identical to
 // STNERF_PREC_FP32_SIMT.
 //
+// STNERF_TRAIN_TC_3XTF32 routes the GEMMs of every layer with 128 or more outputs to the 3xTF32 tensor-core GEMM of
+// mlp_train_tc.cu (same roles, epilogue functors and point chunks; mlp_train.cuh); the 1- and 3-wide heads, the encodings, d_pos,
+// the bias row sums and the chunk reduction run here in both precisions.
+//
 // Weights are the stnerf_load_* blob (state_dict order, nn.Linear (out, in) row-major), read in place; the gradients come
 // back as one blob in the same order.
-#include "common.cuh"
+#include "mlp_train.cuh"
 
 namespace stnerf {
 
@@ -43,61 +47,6 @@ __host__ __device__ constexpr int m_h(int i) { return PE_MOTION + HEAD * (i - 1)
 
 int enc_rows(int use_time) { return PE_DIR + (use_time ? PE_TIME : 0); }
 int s_h8(int use_time) { return S_ENC + enc_rows(use_time); }
-
-// A view of a matrix: element (r, c) at p[r*sr + c*sc]
-struct Mat {
-  const float* p;
-  long long sr, sc;
-  __device__ __forceinline__ float at(long long r, long long c) const { return p[r * sr + c * sc]; }
-};
-
-struct ZeroInit {
-  __device__ __forceinline__ float operator()(int) const { return 0.f; }
-};
-struct BiasInit {
-  const float* b;
-  __device__ __forceinline__ float operator()(int m) const { return __ldg(b + m); }
-};
-
-// forward: output (m, n) -> p[m*sm + n*sn], optionally ReLU'd
-struct Store {
-  float* p;
-  long long sm, sn;
-  int relu;
-  __device__ __forceinline__ void operator()(int m, long long n, float v) const { p[m * sm + n * sn] = relu ? fmaxf(v, 0.f) : v; }
-};
-
-// delta of a layer's input.  Rows m < split are a ReLU output h (saved, pitch P): out = (v [+ ws[m] ds[n]]) where h > 0,
-// else 0.  Rows m >= split belong to PE(pos), which has no ReLU: written to (acc = 0) or added to (acc = 1) enc.
-struct DeltaEpi {
-  float* out;
-  const float* h;
-  long long P;
-  const float* ws;
-  const float* ds;
-  int split;
-  float* enc;
-  int acc;
-  __device__ __forceinline__ void operator()(int m, long long n, float v) const {
-    if (m < split) {
-      if (ws) v = fmaf(__ldg(ws + m), ds[n], v);
-      out[m * P + n] = h[m * P + n] > 0.f ? v : 0.f;
-    } else {
-      float* e = enc + (m - split) * P + n;
-      *e = acc ? *e + v : v;
-    }
-  }
-};
-
-// weight gradient: the partial tile of point chunk blockIdx.z
-struct PartialStore {
-  float* part;
-  int N;
-  long long MN;
-  __device__ __forceinline__ void operator()(int m, long long n, float v) const {
-    part[blockIdx.z * MN + (long long)m * N + n] = v;
-  }
-};
 
 // C(m, n) = init(m) + sum over k in chunk blockIdx.z of A(m, k) B(k, n), k ascending, one fmaf per term; epi(m, n, C).
 // A_KC / B_KC: the operand is contiguous along k (else along m / n), which picks the coalesced tile-load order.
@@ -208,11 +157,17 @@ __global__ void __launch_bounds__(TT) rowsum_kernel(Mat D, long long P, float* _
   if (tid == 0) out[m] = red[0];
 }
 
+// The wide layers (128 or more outputs) run on the 3xTF32 tensor-core GEMM in STNERF_TRAIN_TC_3XTF32; the 1- and 3-wide heads
+// always run on the SIMT GEMM.
+bool on_tc(int prec, int M) { return prec == STNERF_TRAIN_TC_3XTF32 && M >= HEAD; }
+
 // dW (M x N, row-major at dw) = sum_p D(m, p) H(n, p) and db (M) = sum_p D(m, p), for H = saved rows starting at `h`
 template <bool D_KC>
-int weight_grad(Mat D, const float* h, int M, int N, long long P, float* dw, float* db, float* part, cudaStream_t st) {
+int weight_grad(Mat D, const float* h, int M, int N, long long P, float* dw, float* db, float* part, cudaStream_t st,
+                int prec = STNERF_TRAIN_FP32) {
   const long long ch = grad_chunk(P), nz = (P + ch - 1) / ch, MN = (long long)M * N;
-  int rc = gemm<D_KC, true, true>(D, Mat{h, 1, P}, M, N, P, ch, ZeroInit{}, PartialStore{part, N, MN}, st);
+  int rc = (D_KC && on_tc(prec, M)) ? tc_train_wgrad(D.p, h, M, N, P, ch, part, st)
+                                    : gemm<D_KC, true, true>(D, Mat{h, 1, P}, M, N, P, ch, ZeroInit{}, PartialStore{part, N, MN}, st);
   if (rc) return rc;
   reduce_partials_kernel<<<(unsigned)((MN + 255) / 256), 256, 0, st>>>(part, (int)nz, MN, dw);
   STNERF_LAUNCH_CHECK();
@@ -348,12 +303,19 @@ __global__ void spacenet_dpos_kernel(const float* __restrict__ saved, const floa
 unsigned pt_blocks(long long P) { return (unsigned)((P + 255) / 256); }
 
 // forward of one hidden / output layer: out rows = act(W . in rows + b)
-int fwd_layer(const float* W, const Layout& L, int l, const float* in, long long P, Store out, cudaStream_t st) {
+int fwd_layer(const float* W, const Layout& L, int l, const float* in, long long P, Store out, cudaStream_t st,
+              int prec = STNERF_TRAIN_FP32) {
+  if (on_tc(prec, L.nout[l]))      // every wide layer is a ReLU'd hidden layer stored feature-major
+    return tc_train_forward(W + L.w[l], L.kin[l], W + L.b[l], in, L.nout[l], P, out.p, st);
   return gemm<true, false>(Mat{W + L.w[l], L.kin[l], 1}, Mat{in, P, 1}, L.nout[l], P, L.kin[l], L.kin[l],
                            BiasInit{W + L.b[l]}, out, st);
 }
 // delta of layer l's input rows 0..M-1 from the layer's output delta d_out (nout[l] x P, feature-major)
-int delta_layer(const float* W, const Layout& L, int l, const float* d_out, int M, long long P, DeltaEpi epi, cudaStream_t st) {
+int delta_layer(const float* W, const Layout& L, int l, const float* d_out, int M, long long P, DeltaEpi epi, cudaStream_t st,
+                int prec = STNERF_TRAIN_FP32) {
+  if (on_tc(prec, L.nout[l]))
+    return tc_train_delta(W + L.w[l], L.kin[l], L.nout[l], d_out, M, P, epi.out, epi.h, epi.ws, epi.ds, epi.split, epi.enc, epi.acc,
+                          st);
   return gemm<false, false, true>(Mat{W + L.w[l], 1, L.kin[l]}, Mat{d_out, P, 1}, M, P, L.nout[l], L.nout[l], ZeroInit{}, epi,
                                   st);
 }
@@ -370,22 +332,22 @@ size_t train_scratch_bytes(int kind, int /*use_time*/, long long P) {
 }
 
 int launch_spacenet_train_forward(const float* W, int use_time, const float* pos, const float* dirs, const float* times,
-                                  long long P, float* rgb, float* sigma, float* saved, cudaStream_t st) {
+                                  long long P, float* rgb, float* sigma, float* saved, cudaStream_t st, int prec) {
   const Layout L = spacenet_layout(use_time);
   spacenet_encode_kernel<<<pt_blocks(P), 256, 0, st>>>(pos, dirs, times, use_time, P, saved);
   STNERF_LAUNCH_CHECK();
   int rc = 0;
   for (int l = 0; l < 7 && !rc; ++l)                                                       // stage1, stage2 :135-137
-    rc = fwd_layer(W, L, l, saved + S_IN[l] * P, P, Store{saved + S_OUT[l] * P, P, 1, 1}, st);
+    rc = fwd_layer(W, L, l, saved + S_IN[l] * P, P, Store{saved + S_OUT[l] * P, P, 1, 1}, st, prec);
   const int h8 = s_h8(use_time);
   if (!rc) rc = fwd_layer(W, L, 7, saved + S_H7 * P, P, Store{sigma, 0, 1, 0}, st);          // density_net :139
-  if (!rc) rc = fwd_layer(W, L, 8, saved + S_H7 * P, P, Store{saved + h8 * P, P, 1, 1}, st); // rgb_net.1 :143-149
+  if (!rc) rc = fwd_layer(W, L, 8, saved + S_H7 * P, P, Store{saved + h8 * P, P, 1, 1}, st, prec); // rgb_net.1 :143-149
   if (!rc) rc = fwd_layer(W, L, 9, saved + h8 * P, P, Store{rgb, 1, 3, 0}, st);             // rgb_net.3
   return rc;
 }
 
 int launch_spacenet_backward(const float* W, int use_time, long long P, const float* saved, const float* d_rgb,
-                             const float* d_sigma, float* dW, float* d_pos, void* scratch, cudaStream_t st) {
+                             const float* d_sigma, float* dW, float* d_pos, void* scratch, cudaStream_t st, int prec) {
   const Layout L = spacenet_layout(use_time);
   float* D0 = (float*)scratch;
   float* D1 = D0 + HID * P;
@@ -400,21 +362,23 @@ int launch_spacenet_backward(const float* W, int use_time, long long P, const fl
                               DeltaEpi{D1, h8, P, nullptr, nullptr, HEAD, nullptr, 0}, st))) return rc;
   // density_net.0 and rgb_net.1: weights, then delta of h7 from both heads (the direction / time rows get none)
   if ((rc = weight_grad<true>(Mat{d_sigma, 0, 1}, h7, 1, HID, P, dW + L.w[7], dW + L.b[7], part, st))) return rc;
-  if ((rc = weight_grad<true>(Mat{D1, P, 1}, h7, HEAD, L.kin[8], P, dW + L.w[8], dW + L.b[8], part, st))) return rc;
-  if ((rc = delta_layer(W, L, 8, D1, HID, P, DeltaEpi{D0, h7, P, W + L.w[7], d_sigma, HID, nullptr, 0}, st))) return rc;
+  if ((rc = weight_grad<true>(Mat{D1, P, 1}, h7, HEAD, L.kin[8], P, dW + L.w[8], dW + L.b[8], part, st, prec))) return rc;
+  if ((rc = delta_layer(W, L, 8, D1, HID, P, DeltaEpi{D0, h7, P, W + L.w[7], d_sigma, HID, nullptr, 0}, st, prec))) return rc;
   // trunk, top down.  stage2.0's input delta splits at the skip concatenation (:137): rows 0-255 reach h4, rows 256-318
   // reach PE(pos), as does stage1.0's.
   float *cur = D0, *nxt = D1;
   for (int l = 6; l >= 0; --l) {
-    if ((rc = weight_grad<true>(Mat{cur, P, 1}, saved + S_IN[l] * P, HID, L.kin[l], P, dW + L.w[l], dW + L.b[l], part, st)))
+    if ((rc = weight_grad<true>(Mat{cur, P, 1}, saved + S_IN[l] * P, HID, L.kin[l], P, dW + L.w[l], dW + L.b[l], part, st,
+                                prec)))
       return rc;
     if (l > 0) {
       const int M = (l == 4 && d_pos) ? HID + PE_POS : HID;
-      if ((rc = delta_layer(W, L, l, cur, M, P, DeltaEpi{nxt, saved + S_IN[l] * P, P, nullptr, nullptr, HID, dpe, 0}, st)))
+      if ((rc = delta_layer(W, L, l, cur, M, P, DeltaEpi{nxt, saved + S_IN[l] * P, P, nullptr, nullptr, HID, dpe, 0}, st,
+                            prec)))
         return rc;
       float* t = cur; cur = nxt; nxt = t;
     } else if (d_pos) {
-      if ((rc = delta_layer(W, L, 0, cur, PE_POS, P, DeltaEpi{nullptr, nullptr, P, nullptr, nullptr, 0, dpe, 1}, st)))
+      if ((rc = delta_layer(W, L, 0, cur, PE_POS, P, DeltaEpi{nullptr, nullptr, P, nullptr, nullptr, 0, dpe, 1}, st, prec)))
         return rc;
     }
   }
@@ -426,19 +390,19 @@ int launch_spacenet_backward(const float* W, int use_time, long long P, const fl
 }
 
 int launch_motionnet_train_forward(const float* W, const float* xyzt, long long P, const int* lerp_flag, int lerp_force,
-                                   float* flow, float* saved, cudaStream_t st) {
+                                   float* flow, float* saved, cudaStream_t st, int prec) {
   const Layout L = motionnet_layout();
   motionnet_encode_kernel<<<pt_blocks(P), 256, 0, st>>>(xyzt, P, lerp_flag, lerp_force, saved);
   STNERF_LAUNCH_CHECK();
   int rc = 0;
   for (int l = 0; l < 5 && !rc; ++l)                                                        // motion_net.0 .. .8
-    rc = fwd_layer(W, L, l, saved + (l == 0 ? M_PE : m_h(l)) * P, P, Store{saved + m_h(l + 1) * P, P, 1, 1}, st);
+    rc = fwd_layer(W, L, l, saved + (l == 0 ? M_PE : m_h(l)) * P, P, Store{saved + m_h(l + 1) * P, P, 1, 1}, st, prec);
   if (!rc) rc = fwd_layer(W, L, 5, saved + m_h(5) * P, P, Store{flow, 1, 3, 0}, st);         // motion_net.10
   return rc;
 }
 
 int launch_motionnet_backward(const float* W, long long P, const float* saved, const float* d_flow, float* dW, void* scratch,
-                              cudaStream_t st) {
+                              cudaStream_t st, int prec) {
   const Layout L = motionnet_layout();
   float* D0 = (float*)scratch;
   float* D1 = D0 + HEAD * P;
@@ -451,9 +415,10 @@ int launch_motionnet_backward(const float* W, long long P, const float* saved, c
   float *cur = D0, *nxt = D1;
   for (int l = 4; l >= 0; --l) {
     const float* in = saved + (l == 0 ? M_PE : m_h(l)) * P;
-    if ((rc = weight_grad<true>(Mat{cur, P, 1}, in, HEAD, L.kin[l], P, dW + L.w[l], dW + L.b[l], part, st))) return rc;
+    if ((rc = weight_grad<true>(Mat{cur, P, 1}, in, HEAD, L.kin[l], P, dW + L.w[l], dW + L.b[l], part, st, prec))) return rc;
     if (l > 0) {                                            // the encoding of xyzt gets no gradient
-      if ((rc = delta_layer(W, L, l, cur, HEAD, P, DeltaEpi{nxt, in, P, nullptr, nullptr, HEAD, nullptr, 0}, st))) return rc;
+      if ((rc = delta_layer(W, L, l, cur, HEAD, P, DeltaEpi{nxt, in, P, nullptr, nullptr, HEAD, nullptr, 0}, st, prec)))
+        return rc;
       float* t = cur; cur = nxt; nxt = t;
     }
   }

@@ -14,6 +14,16 @@ MAX_S = 512
 PREC_FP32_SIMT, PREC_TC_3XF16, PREC_TC_F16, PREC_TC_MIXED, PREC_TC_3XF16_CF = 0, 1, 2, 3, 4
 PRECISIONS = {"fp32": PREC_FP32_SIMT, "exact": PREC_TC_3XF16, "tc3": PREC_TC_3XF16, "fast": PREC_TC_F16, "mixed": PREC_TC_MIXED,
               "exact_cf": PREC_TC_3XF16_CF}
+# training precision of the differentiable networks (STNERF_TRAIN_*): cfg.MODEL.B200_TRAIN_PRECISION / train_precision=
+TRAIN_FP32, TRAIN_TC_3XTF32 = 0, 1
+TRAIN_PRECISIONS = {"fp32": TRAIN_FP32, "tf32x3": TRAIN_TC_3XTF32}
+
+
+def train_precision_code(name: str) -> int:
+    """STNERF_TRAIN_* value of a training precision name; unknown names raise ValueError."""
+    if name not in TRAIN_PRECISIONS:
+        raise ValueError("unknown training precision %r (one of %s)" % (name, ", ".join(sorted(TRAIN_PRECISIONS))))
+    return TRAIN_PRECISIONS[name]
 
 # STNERF_B200_LIB selects another build of the same ABI (e.g. to compare two builds with scripts/dump_networks.py)
 LIB_PATH = os.environ.get("STNERF_B200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libstnerf_b200.so")
@@ -81,6 +91,11 @@ _SIGNATURES = {
     "stnerf_spacenet_backward": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_size_t, _P]),
     "stnerf_motionnet_train_forward": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, C.c_size_t, _P]),
     "stnerf_motionnet_backward": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, _P]),
+    "stnerf_train_scratch_bytes_prec": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "stnerf_spacenet_train_forward_prec": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int, _P]),
+    "stnerf_spacenet_backward_prec": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P, _P, _P, _P, C.c_size_t, C.c_int, _P]),
+    "stnerf_motionnet_train_forward_prec": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, C.c_size_t, C.c_int, _P]),
+    "stnerf_motionnet_backward_prec": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_size_t, C.c_int, _P]),
     "stnerf_composite_backward": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P, _P, _P, _P, _P, _P]),
     "stnerf_train_sample": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, _P, C.c_uint64, _P, _P, _P, _P, _P, _P]),
     "stnerf_train_points": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P, C.c_int, _P, C.c_int64, _P, _P, _P, _P,

@@ -322,8 +322,10 @@ class LayeredRFRender(torch.nn.Module):
 
 def build_layered_model(cfg, camera_num=0, scale=None, shift=None):
     """modeling/__init__.py:5-7.  cfg.MODEL.B200_TRAINABLE (default False) selects the trainable model
-    (stnerf_b200.train.TrainableLayeredRFRender): network parameters, a differentiable forward."""
+    (stnerf_b200.train.TrainableLayeredRFRender): network parameters, a differentiable forward whose networks train in
+    cfg.MODEL.B200_TRAIN_PRECISION ("fp32", the default, or "tf32x3")."""
     if bool(getattr(cfg.MODEL, "B200_TRAINABLE", False)):
         from .train import TrainableLayeredRFRender
-        return TrainableLayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift)
+        return TrainableLayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift,
+                                        train_precision=getattr(cfg.MODEL, "B200_TRAIN_PRECISION", "fp32"))
     return LayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift)

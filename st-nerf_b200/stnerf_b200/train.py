@@ -7,12 +7,14 @@ optimiser built by solver/build.py sees every network parameter.
 
 `forward` keeps LayeredRFRender's signature and 5-tuple.  With gradients enabled and a parameter that requires one, it runs
 the differentiable forward of layered_rfrender.py:141-734: sampling and ordered hit lists (`stnerf_train_sample`), per layer
-and pass the compact network inputs (`stnerf_train_points`), MotionNet and SpaceNet on the fp32 training kernels
+and pass the compact network inputs (`stnerf_train_points`), MotionNet and SpaceNet on the training kernels
 (`nets.MotionNetFunction` / `nets.SpaceNetFunction`), the masked scatter into the sample grid (`stnerf_train_scatter`, backward
 `stnerf_train_gather`), the per-layer and merged composites (`volume`), and the fine depths from `stnerf_sample_pdf`.  Depths,
-sample points and rays get no gradient, as in the reference (:314-315,461).  Training always runs the fp32 kernels: `precision`
-selects only the render path, which every other call takes (e.g. the evaluator's under `torch.no_grad()`), with the current
-weights -- re-uploaded when a parameter changed since the last upload.
+sample points and rays get no gradient, as in the reference (:314-315,461).  `train_precision` (default
+cfg.MODEL.B200_TRAIN_PRECISION, else "fp32") selects the networks' training kernels and is applied to every network submodule:
+"fp32" on CUDA cores, or "tf32x3" on tensor cores (nets.py).  `precision` selects only the render path, which every other call
+takes (e.g. the evaluator's under `torch.no_grad()`), with the current weights -- re-uploaded when a parameter changed since the
+last upload.
 
 Without injected uniforms both paths draw the same Philox streams, so a grad and a no-grad forward with the same `seed` place
 the same samples.  Identical calls give bit-identical gradients: the hit lists are in ray order and every kernel on the path
@@ -74,15 +76,18 @@ class _ScatterFunction(torch.autograd.Function):
 class TrainableLayeredRFRender(LayeredRFRender):
     """LayeredRFRender with the reference's network submodules and a differentiable forward (module docstring)."""
 
-    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision=None):
+    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision=None, train_precision=None):
         super().__init__(cfg, camera_num=camera_num, scale=scale, shift=shift, precision=precision)
+        tp = train_precision or getattr(cfg.MODEL, "B200_TRAIN_PRECISION", "fp32")
+        L.train_precision_code(tp)
+        self.train_precision = tp
         n = self.layer_num
         # registration order = the reference's (layered_rfrender.py:59-93) = key order of fresh_state_dict / the checkpoints
-        self.spacenets = nn.ModuleList([SpaceNet(use_time=self.use_space_time) for _ in range(n)])
-        self.spacenets_fine = nn.ModuleList([SpaceNet(use_time=self.use_space_time) for _ in range(n)])
-        self.bkgd_spacenet = SpaceNet(use_time=self.bkgd_use_space_time)
-        self.bkgd_spacenet_fine = SpaceNet(use_time=self.bkgd_use_space_time)
-        self.time_deform_nets = nn.ModuleList([MotionNet(c_input=4, input_time=True) for _ in range(n)])
+        self.spacenets = nn.ModuleList([SpaceNet(use_time=self.use_space_time, train_precision=tp) for _ in range(n)])
+        self.spacenets_fine = nn.ModuleList([SpaceNet(use_time=self.use_space_time, train_precision=tp) for _ in range(n)])
+        self.bkgd_spacenet = SpaceNet(use_time=self.bkgd_use_space_time, train_precision=tp)
+        self.bkgd_spacenet_fine = SpaceNet(use_time=self.bkgd_use_space_time, train_precision=tp)
+        self.time_deform_nets = nn.ModuleList([MotionNet(c_input=4, input_time=True, train_precision=tp) for _ in range(n)])
         nn.Module.load_state_dict(self, self._sd)       # the reference's initialisation (fresh_state_dict)
         self._weights_key = None
         self._grad_call = False
@@ -219,13 +224,14 @@ class TrainableLayeredRFRender(LayeredRFRender):
                                             L.ptr(pos), L.ptr(dirs), L.ptr(times), L.ptr(xyzt), L.stream_ptr()),
                 "stnerf_train_points")
         if i > 0:                                                                  # :340-356 / :495-510
-            flow = MotionNetFunction.apply(xyzt, frac, *_params(self.time_deform_nets[i - 1], MOTIONNET_KEYS))
+            mnet = self.time_deform_nets[i - 1]
+            flow = MotionNetFunction.apply(xyzt, frac, mnet.train_precision, *_params(mnet, MOTIONNET_KEYS))
             flow = self._see("flow.%s%d" % ("f" if fine else "c", i), flow)
             pos = xyzt[:, :3] + flow
             net = (self.spacenets_fine if fine else self.spacenets)[i - 1]
         else:
             net = self.bkgd_spacenet_fine if fine else self.bkgd_spacenet
-        rgb_c, sigma_c = SpaceNetFunction.apply(pos, dirs, times, use_time, *_params(net, SPACENET_KEYS))
+        rgb_c, sigma_c = SpaceNetFunction.apply(pos, dirs, times, use_time, net.train_precision, *_params(net, SPACENET_KEYS))
         tag = "%s%d" % ("f" if fine else "c", i)
         rgb_c, sigma_c = self._see("rgb." + tag, rgb_c), self._see("sigma." + tag, sigma_c)
         return _ScatterFunction.apply(rgb_c, sigma_c, nat, i, fine, t, hit, m)
