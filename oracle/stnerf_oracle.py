@@ -101,8 +101,9 @@ def motionnet_forward(w: Dict[str, torch.Tensor], xyzt: torch.Tensor) -> torch.T
 
 
 # --------------------------------------------------------------------------- a3
-def ray_box_intersect(o: torch.Tensor, d: torch.Tensor, bmin: torch.Tensor, bmax: torch.Tensor):
-    """layers/RaySamplePoint.py:8-62.  Returns (t_far, t_near) = (max, 2nd max) of valid face hits."""
+def ray_box_candidates(o: torch.Tensor, d: torch.Tensor, bmin: torch.Tensor, bmax: torch.Tensor) -> torch.Tensor:
+    """layers/RaySamplePoint.py:8-58.  (N,6) face candidates in the order left, right, front, back, bottom, up: the face's t
+    where its hit point lies in the face (inclusive), else -1e3."""
     n = o.shape[0]
     eps = torch.tensor(_EPS64, dtype=F32)
     cand = torch.full((n, 6), -1000.0, dtype=F32)
@@ -116,14 +117,24 @@ def ray_box_intersect(o: torch.Tensor, d: torch.Tensor, bmin: torch.Tensor, bmax
                  (p[:, a2] >= bmin[..., a2]) & (p[:, a2] <= bmax[..., a2])        # :34-51 inclusive
             cand[:, col] = torch.where(ok, t, cand[:, col])
             col += 1
-    top = cand.topk(k=2, dim=-1)[0]                                     # :60
+    return cand
+
+
+def ray_box_intersect(o: torch.Tensor, d: torch.Tensor, bmin: torch.Tensor, bmax: torch.Tensor, cols: int = 6):
+    """layers/RaySamplePoint.py:8-62.  Returns (t_far, t_near) = the top-2 of the face candidates and the -1e3 sentinels of
+    tlist = -1e3 * ones_like(rays) (:53), which has one slot per ray column: ``cols`` is the rays' width, 6 for bare
+    [o, d] rays; rays that carry frame-id columns pass their full width."""
+    cand = ray_box_candidates(o, d, bmin, bmax)
+    tlist = torch.cat([cand, torch.full((o.shape[0], cols - 6), -1000.0, dtype=F32)], 1)
+    top = tlist.topk(k=2, dim=-1)[0]                                    # :60
     return top[:, 0], top[:, 1]
 
 
 # --------------------------------------------------------------------------- a4
-def stratified_samples(o, d, bmin, bmax, n1: int, jitter: torch.Tensor, is_bkgd: bool):
-    """layers/RaySamplePoint.py:85-105.  jitter (N,n1) in [0,1).  Returns t (N,n1), xyz (N,n1,3), mask (N)."""
-    t_far, t_near = ray_box_intersect(o, d, bmin, bmax)
+def stratified_samples(o, d, bmin, bmax, n1: int, jitter: torch.Tensor, is_bkgd: bool, cols: int = 6):
+    """layers/RaySamplePoint.py:85-105.  jitter (N,n1) in [0,1), rays ``cols`` columns wide (see ``ray_box_intersect``).
+    Returns t (N,n1), xyz (N,n1,3), mask (N)."""
+    t_far, t_near = ray_box_intersect(o, d, bmin, bmax, cols)
     start = t_near.clone()
     if is_bkgd:
         start[start <= 0] = 0                                           # :93-95
@@ -302,7 +313,7 @@ def render(nets: dict, scene: dict, rays: torch.Tensor, n1: int, n2: int,
     for i in range(l):
         bmin_i = scene["bmin"][i] if table is None else table[row, i, 0]
         bmax_i = scene["bmax"][i] if table is None else table[row, i, 1]
-        t, xyz, m = stratified_samples(o, d, bmin_i, bmax_i, n1, jitter[i], i == 0)
+        t, xyz, m = stratified_samples(o, d, bmin_i, bmax_i, n1, jitter[i], i == 0, rays.shape[1])
         ts.append(t); masks.append(m)
         xyzs.append(_inverse_edit(xyz, i, scale, shift, pivot, fine=False))
     for i in range(l):

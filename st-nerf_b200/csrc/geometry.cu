@@ -9,11 +9,18 @@ namespace stnerf {
 
 // ---------------------------------------------------------------------------------------------------------
 // a3: layers/RaySamplePoint.py:8-62 -- six slab candidates, inclusive in-face tests, top-2.
+// tlist is -1e3 * ones_like(rays) (:53): one slot per ray COLUMN, six face slots and a -1e3 sentinel per column beyond
+// the sixth, and the top-2 (:60) runs over all of them.  `sentinels` = min(2, columns - 6) is how many of those take
+// part: a 6-column ray has none, so when five or six faces are valid and all lie below -1e3 its top-2 is (-1e3, face) or
+// two faces, where a ray with more columns gets (-1e3, -1e3).
 // ---------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int ray_box_sentinels(int columns) { return min(2, columns - 6); }
+
 __device__ __forceinline__ void ray_box(const float o[3], const float d[3], const float bmin[3], const float bmax[3],
-                                        float& t_far, float& t_near) {
+                                        int sentinels, float& t_far, float& t_near) {
   const float eps = 2.220446049250313e-16f;   // np.finfo(float).eps cast to fp32 (:17-22)
-  float m1 = -1000.0f, m2 = -1000.0f;         // tlist initialised to -1e3 (:53); top-2 over >= 7 columns (:60)
+  // an invalid face is a -1e3 candidate, so the six faces always fill both slots; -inf only marks a missing sentinel
+  float m1 = sentinels > 0 ? -1000.0f : -INFINITY, m2 = sentinels > 1 ? -1000.0f : -INFINITY;
 #pragma unroll
   for (int axis = 0; axis < 3; ++axis) {
     const int a1 = (axis + 1) % 3, a2 = (axis + 2) % 3;
@@ -35,9 +42,9 @@ __device__ __forceinline__ void ray_box(const float o[3], const float d[3], cons
 
 // a4: start / width of the stratified bins of one (ray, box) (layers/RaySamplePoint.py:91-105)
 __device__ __forceinline__ void ray_bins(const float o[3], const float d[3], const float bmin[3], const float bmax[3],
-                                         bool is_bkgd, int n1, float& start, float& width, bool& hit) {
+                                         int sentinels, bool is_bkgd, int n1, float& start, float& width, bool& hit) {
   float t_far, t_near;
-  ray_box(o, d, bmin, bmax, t_far, t_near);
+  ray_box(o, d, bmin, bmax, sentinels, t_far, t_near);
   start = t_near;
   if (is_bkgd && start <= 0.0f) start = 0.0f;     // :93-95
   width = (t_far - start) / (float)n1;             // :100
@@ -74,6 +81,8 @@ sample_kernel(const float* __restrict__ rays, long long n, int ray_stride, const
     d[0] = p[3]; d[1] = p[4]; d[2] = p[5];
   }
   unsigned my_hits = 0;
+  // the rays' columns follow from the scene: [o, d, frame_id] with a shared frame id, else one frame id per layer
+  const int sentinels = ray_box_sentinels(scene.fid_shared ? 7 : 6 + n_layers);
   // rays of a mixed-frame batch: the boxes of the ray's own frame, index_select(frame_id - 1) (layered_rfrender.py:193)
   const float* my_boxes = nullptr;
   if (box_table != nullptr && live) {
@@ -90,7 +99,7 @@ sample_kernel(const float* __restrict__ rays, long long n, int ray_stride, const
     }
     float start, width;
     bool h;
-    ray_bins(o, d, bmin, bmax, i == 0, n1, start, width, h);
+    ray_bins(o, d, bmin, bmax, sentinels, i == 0, n1, start, width, h);
     h = h && live;
     s_start[i][tid] = start;
     s_width[i][tid] = width;
@@ -165,15 +174,16 @@ __global__ void intersect_sample_kernel(const float* __restrict__ rays, long lon
   if (r >= n) return;
   const float* p = rays + r * ray_stride;
   const float o[3] = {p[0], p[1], p[2]}, d[3] = {p[3], p[4], p[5]};
+  const int sentinels = ray_box_sentinels(ray_stride);     // the rays are ray_stride columns wide
   if (tfar_tnear) {
     float tf, tn;
-    ray_box(o, d, box.lo, box.hi, tf, tn);
+    ray_box(o, d, box.lo, box.hi, sentinels, tf, tn);
     tfar_tnear[2 * r] = tf;
     tfar_tnear[2 * r + 1] = tn;
   }
   float start, width;
   bool h;
-  ray_bins(o, d, box.lo, box.hi, is_bkgd != 0, n1, start, width, h);
+  ray_bins(o, d, box.lo, box.hi, sentinels, is_bkgd != 0, n1, start, width, h);
   if (mask) mask[r] = h ? 1 : 0;
   for (int k = 0; k < n1; ++k) {
     const float a = (float)k + jitter[r * n1 + k];
