@@ -223,6 +223,45 @@ int stnerf_spacenet(stnerf_handle h, int layer, int fine, const float* pos, cons
 int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
                      void* stream);
 
+/* ---- geometry: a layer's density field at one frame, and marching cubes ------------------------------------------------------
+ * The field of layer `layer` in pass `fine` (0 coarse nets, 1 fine nets) at frame `frame_id` is what stnerf_render's network for
+ * that layer and pass gives at a world point, in the context's precision and with its scene (stnerf_set_scene):
+ *   1. the pass' inverse edit, rounded as the render rounds it: p -= shift (modeling/layered_rfrender.py:293-298 / :467-471),
+ *      then p = (p - pivot)/scale + pivot with scale_coarse_on (fine = 0, :300-303) or scale_fine_on (fine = 1, :473-475);
+ *   2. a performer (layer >= 1): flow = MotionNet(p, frame_id) and p += flow, one round-to-nearest fp32 add (:340-356 /
+ *      :495-510); the time encoding is lerped exactly when frame_id is fractional (modeling/motion_net.py:53 for one frame);
+ *   3. SpaceNet(p, dir, frame_id) (:397-409 / :552-563): the time input is frame_id when the net consumes time.
+ * Layer and weight errors return STNERF_EINVAL / STNERF_ENOWEIGHTS; a call before stnerf_set_scene returns STNERF_EINVAL.   */
+typedef struct {
+  float origin[3];                               /* point (i,j,k) = origin + (i,j,k)*step: one fp32 product and one fp32 sum  */
+  float step[3];                                 /* per axis, each rounded on its own                                        */
+  int32_t dims[3];                               /* values are [dims0][dims1][dims2], C order, x slowest                      */
+} stnerf_grid;
+/* xyz (P,3) world points, dirs (P,3) view directions -> rgb (P,3) raw logits, sigma (P) raw.  rgb = NULL: sigma only, and dirs
+ * may then be NULL too.  P = 0 succeeds without touching a pointer.  Enqueue only.                                             */
+int stnerf_layer_field(stnerf_handle h, int layer, int fine, float frame_id, const float* xyz, const float* dirs, int64_t P,
+                       float* rgb, float* sigma, void* stream);
+/* The field's sigma on a grid (dims >= 2 per axis, finite origin and steps, else STNERF_EINVAL) -> sigma [dims0][dims1][dims2].
+ * Equal, bit for bit, to stnerf_layer_field on the grid's points.  The grid is evaluated in chunks of 2^20 points in
+ * stream-ordered device scratch of a size that does not depend on dims; enqueue only (no host synchronisation).               */
+int stnerf_layer_grid(stnerf_handle h, int layer, int fine, float frame_id, const stnerf_grid* grid_host, float* sigma,
+                      void* stream);
+/* Marching cubes of a sigma grid (no context; the grid as above, with steps > 0).  A corner is inside when v > level; NaN is
+ * outside.  A vertex lies on every grid edge whose endpoints differ in that test, at p0 + (level - v0)/(v1 - v0)*(p1 - p0) in
+ * fp32 (at the outside endpoint when v0 or v1 is not finite).  Grid point (i,j,k) owns the vertices of its +x, +y, +z edges,
+ * in that order, and vertices are numbered grid-point-major, so neighbouring cells share them: the mesh is indexed.  Triangles
+ * come cell-major from a 256-case table that cuts every ambiguous face the same way from both of its cells (the inside corners
+ * are kept apart), so a surface that stays off the grid border is closed; they are wound so that their normals point from
+ * inside to outside (toward lower values).  Identical calls give identical bits.
+ * Use: scratch of stnerf_mc_scratch_bytes bytes (0 = invalid grid); stnerf_mc_count fills it and returns the vertex and face
+ * counts (one device->host copy: the only host synchronisation; STNERF_EINVAL when the vertex count does not fit int32);
+ * stnerf_mc_fill, with the same sigma, grid, level and scratch, writes verts (V,3) fp32 and faces (F,3) int32.             */
+size_t stnerf_mc_scratch_bytes(const stnerf_grid* grid_host);
+int stnerf_mc_count(const float* sigma, const stnerf_grid* grid_host, float level, void* scratch, size_t scratch_bytes,
+                    int64_t* n_verts_host, int64_t* n_faces_host, void* stream);
+int stnerf_mc_fill(const float* sigma, const stnerf_grid* grid_host, float level, void* scratch, size_t scratch_bytes,
+                   float* verts, int32_t* faces, void* stream);
+
 /* ---- training: differentiable SpaceNet / MotionNet (no context) ------------------------------------------------------------
  * Training precision of the _prec entry points below; the entry points without _prec are STNERF_TRAIN_FP32.               */
 enum {

@@ -1051,6 +1051,87 @@ extern "C" int stnerf_motionnet(stnerf_handle c, int layer, const float* xyzt, i
   return run_motionnet(c, s, net, c->any_frac, lerp_mode, nullptr, flow, st);
 }
 
+// ---- a layer's field at one frame (extract.cu builds the points; the networks are the render's) ------------------------------
+static constexpr long long FIELD_CHUNK = 1LL << 20;
+
+static int field_check(stnerf_ctx* c, int layer, int fine, float frame_id) {
+  if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || !isfinite(frame_id)) return STNERF_EINVAL;
+  if (!c->space[fine][layer].loaded || (layer > 0 && !c->motion[layer].loaded)) return STNERF_ENOWEIGHTS;
+  if (!c->have_scene) return STNERF_EINVAL;
+  int cur = -1;                                       // the context's scene and weights live on the device it was created on
+  STNERF_CUDA(cudaGetDevice(&cur));
+  return cur == c->device ? STNERF_OK : STNERF_EINVAL;
+}
+
+// Points [0, P) of `xyz` (or of grid `g` when xyz == null) through the edit, the MotionNet and the SpaceNet, chunk by chunk.
+static int field_run(stnerf_ctx* c, int layer, int fine, float frame_id, const float* xyz, const FieldGrid& g, long long P,
+                     const float* dirs, float* rgb, float* sigma, cudaStream_t st) {
+  const stnerf_scene& sc = c->scene;
+  FieldEdit e;
+  memset(&e, 0, sizeof(e));
+  e.shift_on = sc.shift_on[layer];
+  e.scale_on = fine ? sc.scale_fine_on[layer] : sc.scale_coarse_on[layer];
+  for (int a = 0; a < 3; ++a) { e.shift[a] = sc.shift[layer][a]; e.pivot[a] = sc.pivot[a]; }
+  e.scale = e.scale_on ? sc.scale[layer] : 1.0f;
+  const int lerp = floorf(frame_id) != frame_id ? 1 : 0;              // motion_net.py:53 for a batch of one frame
+  const long long chunk = std::min(P, FIELD_CHUNK);
+  // stream-ordered scratch: xyzt (chunk,4), deformed points (chunk,3), zero directions (chunk,3) when none are given
+  float* buf = nullptr;
+  STNERF_CUDA(cudaMallocAsync((void**)&buf, (size_t)chunk * 10 * sizeof(float), st));
+  float *xyzt = buf, *def = buf + 4 * chunk, *zdirs = buf + 7 * chunk;
+  int rc = STNERF_OK;
+  if (!dirs && cudaMemsetAsync(zdirs, 0, (size_t)chunk * 3 * sizeof(float), st) != cudaSuccess) rc = STNERF_ECUDA;
+  for (long long p0 = 0; p0 < P && !rc; p0 += chunk) {
+    const long long n = std::min(chunk, P - p0);
+    rc = launch_field_points(xyz, g, p0, n, e, frame_id, xyzt, st);
+    if (!rc && layer > 0) {                                            // :340-356 / :495-510: xyz += MotionNet(xyz, t)
+      PointSrc m;
+      memset(&m, 0, sizeof(m));
+      m.mode = SRC_EXPLICIT; m.pos = xyzt; m.times = xyzt + 3; m.pos_stride = 4; m.time_stride = 4;
+      m.n_slots = n; m.S = 1; m.scale = 1.f;
+      rc = run_motionnet(c, m, c->motion[layer], nullptr, lerp, def, nullptr, st);
+    }
+    if (rc) break;
+    PointSrc s;
+    memset(&s, 0, sizeof(s));
+    s.mode = SRC_EXPLICIT;
+    s.pos = layer > 0 ? def : xyzt; s.pos_stride = layer > 0 ? 3 : 4;
+    s.dirs = dirs ? dirs + 3 * p0 : zdirs;
+    s.times = xyzt + 3; s.time_stride = 4;
+    s.n_slots = n; s.S = 1; s.scale = 1.f;
+    rc = run_spacenet(c, s, c->space[fine][layer], nullptr, rgb ? rgb + 3 * p0 : nullptr, sigma + p0, st);
+  }
+  if (cudaFreeAsync(buf, st) != cudaSuccess && !rc) rc = STNERF_ECUDA;
+  return rc;
+}
+
+extern "C" int stnerf_layer_field(stnerf_handle c, int layer, int fine, float frame_id, const float* xyz, const float* dirs,
+                                  int64_t P, float* rgb, float* sigma, void* stream) {
+  int rc = field_check(c, layer, fine, frame_id);
+  if (rc) return rc;
+  if (P < 0) return STNERF_EINVAL;
+  if (P == 0) return STNERF_OK;
+  if (!xyz || !sigma || (rgb && !dirs)) return STNERF_EINVAL;
+  FieldGrid g;
+  memset(&g, 0, sizeof(g));
+  return field_run(c, layer, fine, frame_id, xyz, g, P, dirs, rgb, sigma, (cudaStream_t)stream);
+}
+
+extern "C" int stnerf_layer_grid(stnerf_handle c, int layer, int fine, float frame_id, const stnerf_grid* grid_host, float* sigma,
+                                 void* stream) {
+  int rc = field_check(c, layer, fine, frame_id);
+  if (rc) return rc;
+  if (!grid_host || !sigma) return STNERF_EINVAL;
+  FieldGrid g;
+  long long P = 1;
+  for (int a = 0; a < 3; ++a) {
+    if (grid_host->dims[a] < 2 || !isfinite(grid_host->origin[a]) || !isfinite(grid_host->step[a])) return STNERF_EINVAL;
+    g.origin[a] = grid_host->origin[a]; g.step[a] = grid_host->step[a]; g.dims[a] = grid_host->dims[a];
+    P *= grid_host->dims[a];
+  }
+  return field_run(c, layer, fine, frame_id, nullptr, g, P, nullptr, nullptr, sigma, (cudaStream_t)stream);
+}
+
 // ---- training: forward with saved activations, and the backward (mlp_train.cu, mlp_train_tc.cu) -----------------------------
 static bool train_prec_ok(int prec) { return prec == STNERF_TRAIN_FP32 || prec == STNERF_TRAIN_TC_3XTF32; }
 

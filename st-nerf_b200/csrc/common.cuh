@@ -246,4 +246,17 @@ int launch_train_gather(int S, const int* hit, long long P, const float* factor,
                         float* d_rgb_c, float* d_sigma_c, cudaStream_t st);
 int launch_train_uniforms(long long n, int n2, int n_layers, uint64_t seed, RayIdMap idmap, float* u, cudaStream_t st);
 
+// extract.cu (a layer's field at one frame; marching cubes)
+struct FieldGrid {           // point (i,j,k) = origin + (i,j,k)*step, one product and one sum per axis
+  float origin[3], step[3];
+  int dims[3];
+};
+struct FieldEdit {           // the inverse edit of one layer and pass (the edit part of march_point)
+  int shift_on, scale_on;
+  float shift[3], scale, pivot[3];
+};
+// n points p0 .. p0+n-1 of `xyz` (P,3), or of the grid when xyz == null, edited -> xyzt (n,4) = (x, y, z, frame)
+int launch_field_points(const float* xyz, const FieldGrid& g, long long p0, long long n, const FieldEdit& e, float frame,
+                        float* xyzt, cudaStream_t st);
+
 }  // namespace stnerf

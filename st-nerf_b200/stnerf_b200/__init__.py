@@ -15,6 +15,8 @@ from .camera_path import CameraPath
 from . import checkpoint_io
 from . import nets
 from . import volume
+from .extract import Mesh, extract_mesh, layer_density, write_ply
 
 __all__ = ["LayeredRFRender", "build_layered_model", "fresh_state_dict", "NativeRenderer", "StnerfError", "ops",
-           "launch_count", "split_planes", "PoseRenderer", "CameraPath", "checkpoint_io", "nets", "volume"]
+           "launch_count", "split_planes", "PoseRenderer", "CameraPath", "checkpoint_io", "nets", "volume",
+           "Mesh", "extract_mesh", "layer_density", "write_ply"]

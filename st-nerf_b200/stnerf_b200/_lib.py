@@ -51,6 +51,11 @@ class View(C.Structure):
                 ("seed", C.c_uint64)]
 
 
+class Grid(C.Structure):
+    """stnerf_grid: point (i,j,k) = origin + (i,j,k)*step, values [dims0][dims1][dims2] (x slowest)."""
+    _fields_ = [("origin", C.c_float * 3), ("step", C.c_float * 3), ("dims", C.c_int32 * 3)]
+
+
 class Profile(C.Structure):
     _fields_ = [("ms", C.c_double * 4), ("points", C.c_double * 4), ("launches", C.c_uint64 * 4)]
 
@@ -85,6 +90,11 @@ _SIGNATURES = {
     "stnerf_positional_encoding": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
     "stnerf_spacenet": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P]),
     "stnerf_motionnet": (C.c_int, [_P, C.c_int, _P, C.c_int64, C.c_int, _P, _P]),
+    "stnerf_layer_field": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int64, _P, _P, _P]),
+    "stnerf_layer_grid": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, C.POINTER(Grid), _P, _P]),
+    "stnerf_mc_scratch_bytes": (C.c_size_t, [C.POINTER(Grid)]),
+    "stnerf_mc_count": (C.c_int, [_P, C.POINTER(Grid), C.c_float, _P, C.c_size_t, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _P]),
+    "stnerf_mc_fill": (C.c_int, [_P, C.POINTER(Grid), C.c_float, _P, C.c_size_t, _P, _P, _P]),
     "stnerf_train_saved_floats": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
     "stnerf_train_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
     "stnerf_spacenet_train_forward": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P, _P]),

@@ -223,6 +223,34 @@ class NativeRenderer:
         del xyzt_c
         return flow
 
+    def layer_field(self, layer: int, fine: bool, frame: float, xyz, dirs=None, want_rgb: bool = True):
+        """The render's field of `layer` (pass `fine`) at frame `frame` at world points xyz (P,3) (stnerf_layer_field):
+        rgb logits (P,3) or None, and raw sigma (P,).  want_rgb=False skips the colour; `dirs` (P,3) is needed otherwise."""
+        xyz_c = _dev_f32(xyz, "xyz")
+        P = xyz_c.shape[0]
+        dirs_c = None if dirs is None else _dev_f32(dirs, "dirs")
+        if want_rgb and dirs_c is None:
+            raise ValueError("layer_field needs view directions for the colour")
+        rgb = torch.empty((P, 3), dtype=torch.float32, device=xyz_c.device) if want_rgb else None
+        sig = torch.empty((P,), dtype=torch.float32, device=xyz_c.device)
+        with torch.cuda.device(xyz_c.device):
+            L.check(L.lib().stnerf_layer_field(self._h, int(layer), 1 if fine else 0, float(frame), L.ptr(xyz_c), L.ptr(dirs_c), P,
+                                               L.ptr(rgb), L.ptr(sig), L.stream_ptr()), "stnerf_layer_field")
+        del xyz_c, dirs_c
+        return rgb, sig
+
+    def layer_grid(self, layer: int, fine: bool, frame: float, origin, step, dims, out: Optional[torch.Tensor] = None):
+        """Raw sigma of the same field on the grid origin + (i,j,k)*step, (dims0, dims1, dims2) (stnerf_layer_grid); enqueue only."""
+        g = make_grid(origin, step, dims)
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if out is None:
+            out = torch.empty(tuple(int(d) for d in dims), dtype=torch.float32, device=dev)
+        assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == tuple(int(d) for d in dims)
+        with torch.cuda.device(out.device):
+            L.check(L.lib().stnerf_layer_grid(self._h, int(layer), 1 if fine else 0, float(frame), C.byref(g), L.ptr(out),
+                                              L.stream_ptr()), "stnerf_layer_grid")
+        return out
+
     def read_depths(self, fine: bool, layer: int, n_rays: int, S: int) -> torch.Tensor:
         """Sample depths (n_rays, S) of `layer` from the last chunk rendered (stnerf_debug_read_depths; parity tooling)."""
         out = torch.empty((n_rays, S), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
@@ -270,6 +298,37 @@ def split_planes(out: torch.Tensor, l: int):
     coarse_layer = [trip(out[0, 1 + i]) for i in range(l)]
     fine_layer = [trip(out[1, 1 + i]) for i in range(l)]
     return fine_mixed, coarse_mixed, fine_layer, coarse_layer
+
+
+def make_grid(origin, step, dims) -> "L.Grid":
+    g = L.Grid()
+    for a in range(3):
+        g.origin[a], g.step[a], g.dims[a] = float(origin[a]), float(step[a]), int(dims[a])
+    return g
+
+
+def marching_cubes(sigma: torch.Tensor, origin, step, level: float):
+    """Indexed triangle mesh of the level set `sigma > level` of a CUDA fp32 grid (D0, D1, D2) whose point (i,j,k) lies at
+    origin + (i,j,k)*step (stnerf_mc_count / stnerf_mc_fill): verts (V,3) fp32 and faces (F,3) int32 on the device."""
+    s = _dev_f32(sigma, "sigma")
+    assert s.dim() == 3, tuple(s.shape)
+    g = make_grid(origin, step, s.shape)
+    lib = L.lib()
+    nbytes = int(lib.stnerf_mc_scratch_bytes(C.byref(g)))
+    if nbytes == 0:
+        raise L.StnerfError("marching_cubes: invalid grid (every dimension >= 2, finite origin, finite positive steps, < 2^31 points)")
+    with torch.cuda.device(s.device):
+        scratch = torch.empty((nbytes,), dtype=torch.uint8, device=s.device)
+        nv, nf = C.c_int64(0), C.c_int64(0)
+        L.check(lib.stnerf_mc_count(L.ptr(s), C.byref(g), float(level), L.ptr(scratch), nbytes, C.byref(nv), C.byref(nf),
+                                    L.stream_ptr()), "stnerf_mc_count")
+        verts = torch.empty((nv.value, 3), dtype=torch.float32, device=s.device)
+        faces = torch.empty((nf.value, 3), dtype=torch.int32, device=s.device)
+        if nv.value > 0:
+            L.check(lib.stnerf_mc_fill(L.ptr(s), C.byref(g), float(level), L.ptr(scratch), nbytes, L.ptr(verts), L.ptr(faces),
+                                       L.stream_ptr()), "stnerf_mc_fill")
+    del s, scratch
+    return verts, faces
 
 
 def launch_count() -> int:

@@ -2,7 +2,8 @@
 
 The reference reads `model.spacenet_fine`, which the layered model does not have (the function is dead code there); here the
 grid is evaluated with the layered model's fine background SpaceNet (layer 0) -- or `layer=i` for performer i -- through
-`stnerf_spacenet`, ReLU applied like the reference (:26)."""
+`stnerf_spacenet`, ReLU applied like the reference (:26).  That is not the density the renderer draws at a frame (no MotionNet,
+no frame id, no scale / shift edit): `stnerf_b200.extract.layer_density` gives that one."""
 import torch
 
 
