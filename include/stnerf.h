@@ -118,6 +118,32 @@ int stnerf_set_scene(stnerf_handle h, const stnerf_scene* scene_host);
  * (int)rays[r][6] - 1 (ids outside [1, n_frames] are clamped; the reference raises).  n_frames = 0 removes the table.      */
 int stnerf_set_box_table(stnerf_handle h, const float* table_host, int n_frames);
 
+/* Per-layer rotation edit.  The reference's LayeredNeuralRenderer takes a `rotation` argument and stores it without using it
+ * (render/layered_neural_renderer.py:19,24); this is the edit it names.  Layer i (0 = background, indexed like shift / scale)
+ * may carry a rotation R_i (fp32 3x3, row-major) about a centre c_i, applied on top of the scale / shift edit:
+ *     world = c + R (edited(p) - c),
+ * so a marched point is first rotated back, p <- c + R^T (p - c), and then goes through the unchanged inverse shift / scale.
+ * The clipping region is the edited box rotated (an oriented box) and the SpaceNet sees the view direction R^T d.
+ * Mechanism: the inverse edit is affine, so a rotated layer samples, marches and looks along its own copy of the rays,
+ *     o' = c + R^T (o - c),   d' = R^T d,   frame-id columns unchanged,
+ * with the op order  q = o - c;  o'_a = ((Rt[a][0] q0 + Rt[a][1] q1) + Rt[a][2] q2) + c_a;  d'_a = (Rt[a][0] d0 + Rt[a][1] d1)
+ * + Rt[a][2] d2  (Rt = R^T, every product and sum rounded on its own).  Depths t stay world depths, so the masks, the
+ * depth-merged composite, the near plane and the Philox keys are unchanged.  A hidden performer is sampled unrotated: hiding a
+ * layer renders the same whether or not it is rotated.
+ * on_host[l]: STNERF_ROT_OFF, STNERF_ROT_CENTRE (rotate about centre_host[i]) or STNERF_ROT_BOX (rotate about the centre of
+ * layer i's box in the scene of each call, (bmin + bmax) * 0.5 in fp32: per view for stnerf_render_views).  R_host [l][9],
+ * centre_host [l][3] (read for STNERF_ROT_CENTRE entries only; may be NULL when there are none).  on_host = NULL clears every
+ * rotation.  Non-finite input or an unknown mode returns STNERF_EINVAL and leaves the rotation as it was.  Host-side only: the
+ * rotation applies to stnerf_render*, stnerf_train_sample / stnerf_train_points and stnerf_layer_field / stnerf_layer_grid.  */
+#define STNERF_ROT_OFF 0
+#define STNERF_ROT_CENTRE 1
+#define STNERF_ROT_BOX 2
+int stnerf_set_rotation(stnerf_handle h, const int32_t* on_host, const float* R_host, const float* centre_host);
+/* The rotated rays of one layer (the kernel every rotated path uses): out (n, ray_stride) = rays with columns 0..5 replaced by
+ * (o', d') as above, for R_host (9, row-major) about centre_host (3).  out must not overlap rays.  Enqueue only.              */
+int stnerf_rotate_rays(const float* rays, int64_t n, int ray_stride, const float* R_host, const float* centre_host, float* out,
+                       void* stream);
+
 /* ---- the hot path: LayeredRFRender.forward (layered_rfrender.py:141-734), BBOX sampling ---------------- */
 /* rays: (n_rays, ray_stride) fp32, columns [o(3), d(3), frame_id_layer0 .. frame_id_layer(l-1)]
  *       (data/datasets/ray_dataset.py:276-281); ray_stride >= 6 + l  (>= 7 with scene.shared_frame_id).

@@ -72,6 +72,9 @@ struct stnerf_ctx {
   bool no_fuse = false;        // STNERF_NO_FUSE=1 in the environment at create: keep the coarse compositing in its own kernel (A/B)
   int* any_frac = nullptr;     // scratch flag for stnerf_motionnet(lerp_mode=-1)
   RayIdMap idmap{0, 0, 0};     // stnerf_set_ray_ids
+  // stnerf_set_rotation: per layer STNERF_ROT_*, R (row-major) and the explicit centre
+  int rot_mode[STNERF_MAX_LAYERS] = {0};
+  float rot_R[STNERF_MAX_LAYERS][9] = {}, rot_c[STNERF_MAX_LAYERS][3] = {};
   // profiling (stnerf_profile_begin / _end): CUDA-event pairs around every launch, on the launching stream
   struct ProfRec { int cls; cudaEvent_t a, b; double points; int count_slot; int S; };
   bool prof_on = false;
@@ -455,6 +458,48 @@ int stnerf_set_scene(stnerf_handle c, const stnerf_scene* s) {
 
 }  // extern "C"
 
+// Layer i's rotation for the scene in effect, or false.  `sampled`: a render / training path, where a hidden performer is sampled
+// unrotated (it draws nothing, and this keeps its samples -- which still take part in the resampling -- those of an unrotated layer).
+static bool layer_rot(const stnerf_ctx* c, int i, bool sampled, RayRot& r) {
+  const int mode = c->rot_mode[i];
+  if (mode == STNERF_ROT_OFF || (sampled && i > 0 && !c->scene.shown[i])) return false;
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) r.Rt[3 * a + b] = c->rot_R[i][3 * b + a];
+  for (int a = 0; a < 3; ++a)
+    r.c[a] = mode == STNERF_ROT_BOX ? (c->scene.bmin[i][a] + c->scene.bmax[i][a]) * 0.5f : c->rot_c[i][a];
+  return true;
+}
+
+// The rotated layers of a render or training call: their rotations and one (rays, ray_stride) copy each, in stream-ordered
+// scratch sized for `cap` rays.  layer_rays() points every other layer at the caller's rays.
+struct RotatedRays {
+  int n = 0, layer[STNERF_MAX_LAYERS];
+  RayRot rot[STNERF_MAX_LAYERS];
+  float* buf = nullptr;
+  long long cap = 0;
+  int stride = 0;
+  cudaStream_t st = nullptr;
+  int init(const stnerf_ctx* c, long long cap_rays, int ray_stride, cudaStream_t s, int only_layer = -1) {
+    st = s; cap = cap_rays; stride = ray_stride;
+    for (int i = 0; i < c->l; ++i)
+      if ((only_layer < 0 || i == only_layer) && layer_rot(c, i, true, rot[n])) layer[n++] = i;
+    if (n > 0 && cap > 0) STNERF_CUDA(cudaMallocAsync((void**)&buf, (size_t)n * cap * stride * sizeof(float), st));
+    return STNERF_OK;
+  }
+  // rotate rays [0, m) (m <= cap) into every copy; lr = where each layer's rays are
+  int rotate(const float* rays, long long m, LayerRays& lr) {
+    for (int i = 0; i < STNERF_MAX_LAYERS; ++i) lr.p[i] = rays;
+    for (int k = 0; k < n; ++k) {
+      float* dst = buf + (size_t)k * cap * stride;
+      const int rc = launch_rotate_rays(rays, m, stride, rot[k], dst, st);
+      if (rc) return rc;
+      lr.p[layer[k]] = dst;
+    }
+    return STNERF_OK;
+  }
+  ~RotatedRays() { if (buf) cudaFreeAsync(buf, st); }
+};
+
 // ---------------------------------------------------------------------------------------------------------
 // one pass of the networks over a chunk
 // ---------------------------------------------------------------------------------------------------------
@@ -494,7 +539,7 @@ static int run_motionnet(stnerf_ctx* c, const PointSrc& src, MotionNetDev& net, 
 // `want_raw`: the (rgb, sigma) samples must reach HBM (a later kernel composites them); false only with `fuse`.
 // `reuse_n1` > 0 (fine pass): the MotionNet runs on the S - reuse_n1 NEW depths only; the flow of the coarse depths is the coarse
 // pass' (xyz_coarse), stitched together through the origin map the merge wrote (z_new / src_map).
-static int run_nets(stnerf_ctx* c, const float* rays, long long n, int ray_stride, bool fine, int S, cudaStream_t st,
+static int run_nets(stnerf_ctx* c, const LayerRays& rays, long long n, int ray_stride, bool fine, int S, cudaStream_t st,
                     int chunk_slot, const FuseCoarse* fuse = nullptr, bool want_raw = true, float* coarse_imgs = nullptr,
                     long long plane = 0, int reuse_n1 = 0) {
   const long long R = c->chunk_rays;
@@ -506,7 +551,7 @@ static int run_nets(stnerf_ctx* c, const float* rays, long long n, int ray_strid
     PointSrc s;
     memset(&s, 0, sizeof(s));
     s.mode = SRC_MARCH;
-    s.rays = rays; s.ray_stride = ray_stride;
+    s.rays = rays.p[i]; s.ray_stride = ray_stride;                // a rotated layer marches along its own rays
     s.t = tbuf + i * tl;
     s.S = S; s.layer = c->scene.shared_frame_id ? 0 : i;      // frame-id column offset of this layer
     s.pos_stride = 3; s.time_stride = 1;
@@ -597,6 +642,9 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
   if (rc) return rc;
   const int l = c->l, S2 = n1 + n2;
   const long long R = c->chunk_rays, N = n_rays;
+  RotatedRays rot;
+  rc = rot.init(c, std::min(R, N), ray_stride, st);
+  if (rc) return rc;
   for (long long c0 = 0; c0 < N; c0 += R) {
     const long long n = std::min(R, N - c0);
     if (before_chunk) { rc = before_chunk->fn(before_chunk->user, c0, n, st); if (rc) return rc; }
@@ -607,10 +655,14 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
     uint8_t* mask = ray_mask ? ray_mask + c0 : c->mask_ws;
     const long long mask_ls = ray_mask ? N : R;
     int chunk_slot = -1;
+    LayerRays lr;
     {
       ProfScope ps(c, 2, (double)n, -1, 1, st);
+      rc = rot.rotate(rch, n, lr);
+      if (rc) return rc;
       rc = launch_sample(rch, n, ray_stride, c->dscene, l, n1, jitter ? jitter + c0 * n1 : nullptr, N * n1, seed, c0, c->idmap,
-                         c->t_coarse, R * c->cap_n1, mask, mask_ls, c->hit, R, c->counts, c->lerp_flags, st, c->box_table, c->box_frames);
+                         c->t_coarse, R * c->cap_n1, mask, mask_ls, c->hit, R, c->counts, c->lerp_flags, st, c->box_table, c->box_frames,
+                         &lr);
       if (rc) return rc;
     }
     if (c->prof_on && c->prof_counts && c->prof_chunks < PROF_MAX_CHUNKS) {
@@ -641,7 +693,7 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
       ft.n_total = N; ft.pixels = out.pixels; ft.near_plane = c->dscene.near_plane; ft.thr = c->dscene.thr_layer;
       ft.boarder = c->dscene.boarder; ft.apply_thr = c->dscene.apply_thr;
     }
-    rc = run_nets(c, rch, n, ray_stride, false, n1, st, chunk_slot, fuse ? &ft : nullptr, /*want_raw=*/!fuse || out.coarse != nullptr,
+    rc = run_nets(c, lr, n, ray_stride, false, n1, st, chunk_slot, fuse ? &ft : nullptr, /*want_raw=*/!fuse || out.coarse != nullptr,
                   out.coarse, 5 * N);
     if (rc) return rc;
     CompositeArgs a;
@@ -661,7 +713,7 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
       if (rc) return rc;
     }
     if (n2 > 0) {
-      rc = run_nets(c, rch, n, ray_stride, true, S2, st, chunk_slot, nullptr, true, nullptr, 0, reuse ? n1 : 0);
+      rc = run_nets(c, lr, n, ray_stride, true, S2, st, chunk_slot, nullptr, true, nullptr, 0, reuse ? n1 : 0);
       if (rc) return rc;
       a.t = c->t_fine; a.t_layer_stride = R * c->cap_s2;
       a.raw = c->raw_fine; a.raw_layer_stride = R * c->cap_s2 * 4;
@@ -908,6 +960,46 @@ int stnerf_set_ray_ids(stnerf_handle c, int64_t base, int32_t width, int64_t row
   return STNERF_OK;
 }
 
+int stnerf_set_rotation(stnerf_handle c, const int32_t* on_host, const float* R_host, const float* centre_host) {
+  if (!c) return STNERF_EINVAL;
+  int mode[STNERF_MAX_LAYERS] = {0};
+  float R[STNERF_MAX_LAYERS][9] = {}, cen[STNERF_MAX_LAYERS][3] = {};
+  if (on_host) {                                       // validate everything before changing anything
+    for (int i = 0; i < c->l; ++i) {
+      mode[i] = on_host[i];
+      if (mode[i] < STNERF_ROT_OFF || mode[i] > STNERF_ROT_BOX) return STNERF_EINVAL;
+      if (mode[i] == STNERF_ROT_OFF) continue;
+      if (!R_host || (mode[i] == STNERF_ROT_CENTRE && !centre_host)) return STNERF_EINVAL;
+      for (int k = 0; k < 9; ++k) {
+        R[i][k] = R_host[9 * i + k];
+        if (!isfinite(R[i][k])) return STNERF_EINVAL;
+      }
+      if (mode[i] == STNERF_ROT_CENTRE)
+        for (int a = 0; a < 3; ++a) {
+          cen[i][a] = centre_host[3 * i + a];
+          if (!isfinite(cen[i][a])) return STNERF_EINVAL;
+        }
+    }
+  }
+  memcpy(c->rot_mode, mode, sizeof(mode));
+  memcpy(c->rot_R, R, sizeof(R));
+  memcpy(c->rot_c, cen, sizeof(cen));
+  return STNERF_OK;
+}
+
+int stnerf_rotate_rays(const float* rays, int64_t n, int ray_stride, const float* R_host, const float* centre_host, float* out,
+                       void* stream) {
+  if (n < 0 || ray_stride < 6 || !R_host || !centre_host) return STNERF_EINVAL;
+  if (n == 0) return STNERF_OK;
+  if (!rays || !out) return STNERF_EINVAL;
+  RayRot r;
+  for (int a = 0; a < 3; ++a) {
+    for (int b = 0; b < 3; ++b) r.Rt[3 * a + b] = R_host[3 * b + a];
+    r.c[a] = centre_host[a];
+  }
+  return launch_rotate_rays(rays, n, ray_stride, r, out, (cudaStream_t)stream);
+}
+
 int stnerf_selftest_umma(float* max_err_host) {
   if (!max_err_host) return STNERF_EINVAL;
   return tc_selftest(max_err_host);
@@ -1073,17 +1165,20 @@ static int field_run(stnerf_ctx* c, int layer, int fine, float frame_id, const f
   e.scale_on = fine ? sc.scale_fine_on[layer] : sc.scale_coarse_on[layer];
   for (int a = 0; a < 3; ++a) { e.shift[a] = sc.shift[layer][a]; e.pivot[a] = sc.pivot[a]; }
   e.scale = e.scale_on ? sc.scale[layer] : 1.0f;
+  e.rot_on = layer_rot(c, layer, false, e.rot) ? 1 : 0;
+  const bool rot_dirs = e.rot_on && dirs;                             // the SpaceNet looks along R^T dir
   const int lerp = floorf(frame_id) != frame_id ? 1 : 0;              // motion_net.py:53 for a batch of one frame
   const long long chunk = std::min(P, FIELD_CHUNK);
-  // stream-ordered scratch: xyzt (chunk,4), deformed points (chunk,3), zero directions (chunk,3) when none are given
+  // stream-ordered scratch: xyzt (chunk,4), deformed points (chunk,3), zero directions (chunk,3) when none are given,
+  // rotated directions (chunk,3) for a rotated layer
   float* buf = nullptr;
-  STNERF_CUDA(cudaMallocAsync((void**)&buf, (size_t)chunk * 10 * sizeof(float), st));
-  float *xyzt = buf, *def = buf + 4 * chunk, *zdirs = buf + 7 * chunk;
+  STNERF_CUDA(cudaMallocAsync((void**)&buf, (size_t)chunk * (rot_dirs ? 13 : 10) * sizeof(float), st));
+  float *xyzt = buf, *def = buf + 4 * chunk, *zdirs = buf + 7 * chunk, *rdirs = buf + 10 * chunk;
   int rc = STNERF_OK;
   if (!dirs && cudaMemsetAsync(zdirs, 0, (size_t)chunk * 3 * sizeof(float), st) != cudaSuccess) rc = STNERF_ECUDA;
   for (long long p0 = 0; p0 < P && !rc; p0 += chunk) {
     const long long n = std::min(chunk, P - p0);
-    rc = launch_field_points(xyz, g, p0, n, e, frame_id, xyzt, st);
+    rc = launch_field_points(xyz, g, p0, n, e, frame_id, xyzt, dirs, rdirs, st);
     if (!rc && layer > 0) {                                            // :340-356 / :495-510: xyz += MotionNet(xyz, t)
       PointSrc m;
       memset(&m, 0, sizeof(m));
@@ -1096,7 +1191,7 @@ static int field_run(stnerf_ctx* c, int layer, int fine, float frame_id, const f
     memset(&s, 0, sizeof(s));
     s.mode = SRC_EXPLICIT;
     s.pos = layer > 0 ? def : xyzt; s.pos_stride = layer > 0 ? 3 : 4;
-    s.dirs = dirs ? dirs + 3 * p0 : zdirs;
+    s.dirs = rot_dirs ? rdirs : dirs ? dirs + 3 * p0 : zdirs;
     s.times = xyzt + 3; s.time_stride = 4;
     s.n_slots = n; s.S = 1; s.scale = 1.f;
     rc = run_spacenet(c, s, c->space[fine][layer], nullptr, rgb ? rgb + 3 * p0 : nullptr, sigma + p0, st);
@@ -1270,9 +1365,17 @@ int stnerf_train_sample(stnerf_handle c, const float* rays, int64_t n, int ray_s
   int* counts = scratch;                              // sample_kernel's own (unordered) counters, then the ordered totals
   int* lerp = scratch + STNERF_MAX_LAYERS;
   STNERF_CUDA(cudaMemsetAsync(scratch, 0, 2 * STNERF_MAX_LAYERS * sizeof(int), st));
-  // sampling as in render_core; its block-ordered hit lists land in `hit` and are overwritten in ray order below
-  rc = launch_sample(rays, n, ray_stride, c->dscene, c->l, n1, jitter, n * n1, seed, 0, c->idmap, t, n * n1, mask, n, hit, n,
-                     counts, lerp, st, c->box_table, c->box_frames);
+  // sampling as in render_core (rotated layers along their own rays); its block-ordered hit lists land in `hit` and are
+  // overwritten in ray order below
+  LayerRays lr;
+  {
+    RotatedRays rot;
+    rc = rot.init(c, n, ray_stride, st);
+    if (!rc) rc = rot.rotate(rays, n, lr);
+    if (!rc)
+      rc = launch_sample(rays, n, ray_stride, c->dscene, c->l, n1, jitter, n * n1, seed, 0, c->idmap, t, n * n1, mask, n, hit, n,
+                         counts, lerp, st, c->box_table, c->box_frames, &lr);
+  }
   if (!rc) rc = launch_train_hits(mask, n, c->l, rays, ray_stride, c->scene.shared_frame_id, hit,
                                   scratch + 2 * STNERF_MAX_LAYERS, counts, st);
   int host[2 * STNERF_MAX_LAYERS];
@@ -1297,6 +1400,13 @@ int stnerf_train_points(stnerf_handle c, int layer, int fine, const float* rays,
   s.mode = SRC_MARCH; s.rays = rays; s.ray_stride = ray_stride; s.t = t; s.S = S; s.hit = hit; s.n_slots = m;
   s.layer = c->scene.shared_frame_id ? 0 : layer;
   fill_edit(s, c->scene, layer, fine != 0);
+  // a rotated layer: the points and directions of its own rays, as render_core marches them
+  RotatedRays rot;
+  rc = rot.init(c, n, ray_stride, (cudaStream_t)stream, layer);
+  LayerRays lr;
+  if (!rc) rc = rot.rotate(rays, n, lr);
+  if (rc) return rc;
+  s.rays = lr.p[layer];
   return launch_train_points(s, (long long)m * S, pos, dirs, times, xyzt, (cudaStream_t)stream);
 }
 

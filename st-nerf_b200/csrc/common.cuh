@@ -112,6 +112,30 @@ __device__ __forceinline__ long long src_num_points(const PointSrc& s) {
   return slots * (long long)s.S;
 }
 
+// The rotation edit of one layer (stnerf_set_rotation): Rt = R^T row-major, about centre c.  A rotated layer's ray is
+// o' = c + R^T (o - c), d' = R^T d, each product and sum rounded on its own in this order (include/stnerf.h), so a host
+// restatement in fp32 gives the same bits.  The same map takes a world point of the field (extract.cu) back into the layer.
+struct RayRot {
+  float Rt[9], c[3];
+};
+__device__ __forceinline__ void rotate_back_point(const RayRot& r, const float p[3], float out[3]) {
+  const float q0 = __fsub_rn(p[0], r.c[0]), q1 = __fsub_rn(p[1], r.c[1]), q2 = __fsub_rn(p[2], r.c[2]);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    out[a] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r.Rt[3 * a], q0), __fmul_rn(r.Rt[3 * a + 1], q1)), __fmul_rn(r.Rt[3 * a + 2], q2)),
+                       r.c[a]);
+}
+__device__ __forceinline__ void rotate_back_dir(const RayRot& r, const float d[3], float out[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    out[a] = __fadd_rn(__fadd_rn(__fmul_rn(r.Rt[3 * a], d[0]), __fmul_rn(r.Rt[3 * a + 1], d[1])), __fmul_rn(r.Rt[3 * a + 2], d[2]));
+}
+
+// The rays each layer samples along: p[i] = the caller's rays, or layer i's rotated copy (same stride, same frame ids).
+struct LayerRays {
+  const float* p[STNERF_MAX_LAYERS];
+};
+
 // Maps a ray's index within a call to the id that keys the Philox stream (identity by default).  A caller that renders
 // an image in row-interleaved shards sets (base, width, row_stride) so every pixel draws the same uniforms as in an
 // unsharded render:  id = base + (j / width) * row_stride + (j % width).
@@ -169,7 +193,9 @@ int launch_sample(const float* rays, long long n, int ray_stride, const DevScene
                   const float* jitter, long long jitter_layer_stride, uint64_t seed, long long ray_base, RayIdMap idmap,
                   float* t_coarse, long long t_layer_stride, uint8_t* mask, long long mask_layer_stride,
                   int* hit, long long hit_layer_stride, int* counts, int* lerp_flags, cudaStream_t st,
-                  const float* box_table = nullptr, int n_frames = 0);
+                  const float* box_table = nullptr, int n_frames = 0, const LayerRays* layer_rays = nullptr);
+// out (n, ray_stride) = rays with columns 0..5 replaced by the rotated (o', d'); the frame-id columns copied
+int launch_rotate_rays(const float* rays, long long n, int ray_stride, const RayRot& r, float* out, cudaStream_t st);
 int launch_intersect_sample(const float* rays, long long n, int ray_stride, const float* bmin, const float* bmax,
                             int is_bkgd, int n1, const float* jitter, float* t, float* xyz, uint8_t* mask,
                             float* tfar_tnear, cudaStream_t st);
@@ -251,12 +277,14 @@ struct FieldGrid {           // point (i,j,k) = origin + (i,j,k)*step, one produ
   float origin[3], step[3];
   int dims[3];
 };
-struct FieldEdit {           // the inverse edit of one layer and pass (the edit part of march_point)
-  int shift_on, scale_on;
+struct FieldEdit {           // the inverse edit of one layer and pass (the edit part of march_point), rotation first
+  int shift_on, scale_on, rot_on;
   float shift[3], scale, pivot[3];
+  RayRot rot;
 };
-// n points p0 .. p0+n-1 of `xyz` (P,3), or of the grid when xyz == null, edited -> xyzt (n,4) = (x, y, z, frame)
+// n points p0 .. p0+n-1 of `xyz` (P,3), or of the grid when xyz == null, edited -> xyzt (n,4) = (x, y, z, frame).
+// With e.rot_on and dirs != null, also rdirs (n,3) = R^T dirs[p0 ..].
 int launch_field_points(const float* xyz, const FieldGrid& g, long long p0, long long n, const FieldEdit& e, float frame,
-                        float* xyzt, cudaStream_t st);
+                        float* xyzt, const float* dirs, float* rdirs, cudaStream_t st);
 
 }  // namespace stnerf

@@ -25,7 +25,7 @@ constexpr int EX_BLOCK = 256;
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(EX_BLOCK)
 field_points_kernel(const float* __restrict__ xyz, FieldGrid g, long long p0, long long n, FieldEdit e, float frame,
-                    float* __restrict__ xyzt) {
+                    float* __restrict__ xyzt, const float* __restrict__ dirs, float* __restrict__ rdirs) {
   const long long j = (long long)blockIdx.x * EX_BLOCK + threadIdx.x;
   if (j >= n) return;
   const long long p = p0 + j;
@@ -38,6 +38,17 @@ field_points_kernel(const float* __restrict__ xyz, FieldGrid g, long long p0, lo
 #pragma unroll
     for (int a = 0; a < 3; ++a) v[a] = __fadd_rn(__fmul_rn((float)idx[a], g.step[a]), g.origin[a]);
   }
+  // a rotated layer: back into the layer first, with the op order of rotate_rays_kernel (the render's o' = c + R^T (o - c))
+  if (e.rot_on) {
+    const float w[3] = {v[0], v[1], v[2]};
+    rotate_back_point(e.rot, w, v);
+    if (dirs) {
+      const float d[3] = {dirs[3 * p], dirs[3 * p + 1], dirs[3 * p + 2]};
+      float d2[3];
+      rotate_back_dir(e.rot, d, d2);
+      rdirs[3 * j] = d2[0]; rdirs[3 * j + 1] = d2[1]; rdirs[3 * j + 2] = d2[2];
+    }
+  }
   // the edit part of march_point: p -= shift (layered_rfrender.py:298 / :471); p = (p - pivot)/scale + pivot (:303 / :475)
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
@@ -48,9 +59,10 @@ field_points_kernel(const float* __restrict__ xyz, FieldGrid g, long long p0, lo
 }
 
 int launch_field_points(const float* xyz, const FieldGrid& g, long long p0, long long n, const FieldEdit& e, float frame,
-                        float* xyzt, cudaStream_t st) {
+                        float* xyzt, const float* dirs, float* rdirs, cudaStream_t st) {
   if (n <= 0) return STNERF_OK;
-  field_points_kernel<<<(unsigned)((n + EX_BLOCK - 1) / EX_BLOCK), EX_BLOCK, 0, st>>>(xyz, g, p0, n, e, frame, xyzt);
+  field_points_kernel<<<(unsigned)((n + EX_BLOCK - 1) / EX_BLOCK), EX_BLOCK, 0, st>>>(xyz, g, p0, n, e, frame, xyzt,
+                                                                                     e.rot_on ? dirs : nullptr, rdirs);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
 }

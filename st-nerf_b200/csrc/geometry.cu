@@ -63,7 +63,7 @@ sample_kernel(const float* __restrict__ rays, long long n, int ray_stride, const
               int n_layers, int n1, const float* __restrict__ jitter, long long jitter_layer_stride, uint64_t seed,
               long long ray_base, RayIdMap idmap, float* __restrict__ t_out, long long t_layer_stride, uint8_t* __restrict__ mask,
               long long mask_layer_stride, int* __restrict__ hit, long long hit_layer_stride, int* __restrict__ counts,
-              int* __restrict__ lerp_flags, const float* __restrict__ box_table, int n_frames) {
+              int* __restrict__ lerp_flags, const float* __restrict__ box_table, int n_frames, const __grid_constant__ LayerRays lrays) {
   __shared__ float s_start[STNERF_MAX_LAYERS][SAMPLE_BLOCK];
   __shared__ float s_width[STNERF_MAX_LAYERS][SAMPLE_BLOCK];
   __shared__ int s_warp_hits[STNERF_MAX_LAYERS][SAMPLE_BLOCK / 32];
@@ -99,7 +99,17 @@ sample_kernel(const float* __restrict__ rays, long long n, int ray_stride, const
     }
     float start, width;
     bool h;
-    ray_bins(o, d, bmin, bmax, sentinels, i == 0, n1, start, width, h);
+    if (lrays.p[i] != rays) {         // a rotated layer: its own ray against the unrotated box == the oriented-box clip
+      float oi[3] = {0, 0, 0}, di[3] = {0, 0, 1};
+      if (live) {
+        const float* q = lrays.p[i] + r * ray_stride;
+        oi[0] = q[0]; oi[1] = q[1]; oi[2] = q[2];
+        di[0] = q[3]; di[1] = q[4]; di[2] = q[5];
+      }
+      ray_bins(oi, di, bmin, bmax, sentinels, i == 0, n1, start, width, h);
+    } else {
+      ray_bins(o, d, bmin, bmax, sentinels, i == 0, n1, start, width, h);
+    }
     h = h && live;
     s_start[i][tid] = start;
     s_width[i][tid] = width;
@@ -150,13 +160,42 @@ int launch_sample(const float* rays, long long n, int ray_stride, const DevScene
                   const float* jitter, long long jitter_layer_stride, uint64_t seed, long long ray_base, RayIdMap idmap,
                   float* t_coarse, long long t_layer_stride, uint8_t* mask, long long mask_layer_stride, int* hit,
                   long long hit_layer_stride, int* counts, int* lerp_flags, cudaStream_t st, const float* box_table,
-                  int n_frames) {
+                  int n_frames, const LayerRays* layer_rays) {
   if (n <= 0) return STNERF_OK;
   const int grid = (int)((n + SAMPLE_BLOCK - 1) / SAMPLE_BLOCK);
+  LayerRays lr;
+  for (int i = 0; i < STNERF_MAX_LAYERS; ++i) lr.p[i] = layer_rays ? layer_rays->p[i] : rays;
   sample_kernel<<<grid, SAMPLE_BLOCK, 0, st>>>(rays, n, ray_stride, scene, n_layers, n1, jitter,
                                                jitter_layer_stride, seed, ray_base, idmap, t_coarse, t_layer_stride, mask,
                                                mask_layer_stride, hit, hit_layer_stride, counts, lerp_flags,
-                                               (scene.fid_shared && n_frames > 0) ? box_table : nullptr, n_frames);
+                                               (scene.fid_shared && n_frames > 0) ? box_table : nullptr, n_frames, lr);
+  STNERF_LAUNCH_CHECK();
+  return STNERF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// The rays of a rotated layer (include/stnerf.h: stnerf_set_rotation): o' = c + R^T (o - c), d' = R^T d, frame ids copied.
+// One thread per ray; a full-stride copy, so every consumer indexes it exactly like the caller's rays.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void rotate_rays_kernel(const float* __restrict__ rays, long long n, int ray_stride, const RayRot rot,
+                                   float* __restrict__ out) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const float* p = rays + r * ray_stride;
+  float* q = out + r * ray_stride;
+  const float o[3] = {p[0], p[1], p[2]}, d[3] = {p[3], p[4], p[5]};
+  float o2[3], d2[3];
+  rotate_back_point(rot, o, o2);
+  rotate_back_dir(rot, d, d2);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) { q[a] = o2[a]; q[3 + a] = d2[a]; }
+  for (int k = 6; k < ray_stride; ++k) q[k] = p[k];
+}
+
+int launch_rotate_rays(const float* rays, long long n, int ray_stride, const RayRot& r, float* out, cudaStream_t st) {
+  if (n <= 0) return STNERF_OK;
+  const int block = 256;
+  rotate_rays_kernel<<<(unsigned)((n + block - 1) / block), block, 0, st>>>(rays, n, ray_stride, r, out);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
 }

@@ -89,6 +89,12 @@ class LayeredNeuralRenderer(CameraPath):
             model.cuda()
         return dataset, model
 
+    def set_rotation(self, rotation):
+        """Rotate layers: one entry per layer incl. the background, each None, a 3x3 matrix, a rotation vector (axis * angle,
+        radians) or (R, centre) (stnerf_b200.rotation).  The constructor's `rotation` is stored and unused, as in the
+        reference; this is the call that turns performers."""
+        self.model.rotation = rotation
+
     # ---- layer display: renderer and model stay in step (:653-664) ----------------------------------------------------------
     def hide_layer(self, layer_id):
         self.model.hide_layer(layer_id)

@@ -11,6 +11,9 @@ MAX_LAYERS = 8
 MAX_N1 = 128
 MAX_S = 512
 
+# stnerf_set_rotation modes: no rotation, about an explicit centre, about the centre of the layer's box in each call's scene
+ROT_OFF, ROT_CENTRE, ROT_BOX = 0, 1, 2
+
 PREC_FP32_SIMT, PREC_TC_3XF16, PREC_TC_F16, PREC_TC_MIXED, PREC_TC_3XF16_CF = 0, 1, 2, 3, 4
 PRECISIONS = {"fp32": PREC_FP32_SIMT, "exact": PREC_TC_3XF16, "tc3": PREC_TC_3XF16, "fast": PREC_TC_F16, "mixed": PREC_TC_MIXED,
               "exact_cf": PREC_TC_3XF16_CF}
@@ -75,6 +78,8 @@ _SIGNATURES = {
     "stnerf_weights_import": (C.c_int, [_P, _P, C.c_size_t]),
     "stnerf_set_scene": (C.c_int, [_P, C.POINTER(Scene)]),
     "stnerf_set_box_table": (C.c_int, [_P, _P, C.c_int]),
+    "stnerf_set_rotation": (C.c_int, [_P, _P, _P, _P]),
+    "stnerf_rotate_rays": (C.c_int, [_P, C.c_int64, C.c_int, _P, _P, _P, _P]),
     "stnerf_render": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_uint64, _P, _P, _P]),
     "stnerf_render_host": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, _P, _P]),
     "stnerf_reserve_host": (C.c_int, [_P, C.c_int64, C.c_int]),

@@ -18,6 +18,7 @@ from typing import NamedTuple, Optional, Tuple
 import numpy as np
 import torch
 
+from . import rotation as ROT
 from .native import marching_cubes
 
 
@@ -49,11 +50,13 @@ def _scene_at(model, frame: float):
     nat = model._ensure_native(torch.device("cuda", torch.cuda.current_device()))
     scene = _scene(model, frame)
     nat.set_scene(scene)
+    model._upload_rotation(nat)
     return nat, scene
 
 
 def layer_box(model, layer: int, frame: float):
-    """(lo, hi) corners of the box the render clips `layer` against at `frame` (layer 0: the background box), after edits."""
+    """(lo, hi) corners of the box the render clips `layer` against at `frame` (layer 0: the background box), after the scale /
+    shift edits; a rotated layer clips against this box turned by its rotation (see `layer_density`)."""
     scene = _scene(model, frame)
     return tuple(float(v) for v in scene.bmin[layer]), tuple(float(v) for v in scene.bmax[layer])
 
@@ -74,11 +77,15 @@ def _bbox(bbox):
 
 def layer_density(model, layer: int, frame: float, resolution=128, bbox=None, fine: bool = True) -> LayerDensity:
     """Raw sigma of `layer` at `frame` on a resolution^3 (or R0 x R1 x R2) grid spanning `bbox` -- any corner set, e.g. (2,3)
-    or (8,3) -- or, by default, the layer's box at that frame as the render clips it.  fine=False: the coarse networks."""
+    or (8,3) -- or, by default, the layer's box at that frame as the render clips it (for a rotated layer the world bounds of
+    the turned box, rounded outward).  fine=False: the coarse networks."""
     if not 0 <= int(layer) <= model.layer_num:
         raise ValueError("layer %d out of range [0, %d]" % (layer, model.layer_num))
     nat, scene = _scene_at(model, frame)
     lo, hi = _bbox(bbox) if bbox is not None else (tuple(scene.bmin[layer]), tuple(scene.bmax[layer]))
+    entry = model._rotation_entries()[int(layer)]
+    if bbox is None and entry is not None:
+        lo, hi = ROT.oriented_box_aabb(lo, hi, entry[0], ROT.centre_of(entry, lo, hi))
     origin, step, dims = _grid(lo, hi, resolution)
     sigma = nat.layer_grid(int(layer), bool(fine), float(frame), origin, step, dims)
     return LayerDensity(sigma, origin, step)

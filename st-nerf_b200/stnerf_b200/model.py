@@ -17,6 +17,7 @@ from typing import List, Optional
 import torch
 
 from . import _lib as L
+from . import rotation as ROT
 from .native import NativeRenderer, split_planes
 
 _SPACE_SHAPES = [("stage1.0", 256, 63), ("stage1.2", 256, 256), ("stage1.4", 256, 256), ("stage1.6", 256, 256),
@@ -66,7 +67,7 @@ def fresh_state_dict(layer_num: int, use_space_time: bool, bkgd_use_space_time: 
 class LayeredRFRender(torch.nn.Module):
     """Drop-in for modeling.layered_rfrender.LayeredRFRender at render time (BBOX sampling, retiming rays)."""
 
-    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision: Optional[str] = None):
+    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision: Optional[str] = None, rotation=None):
         super().__init__()
         M = cfg.MODEL
         if M.SAMPLE_METHOD != "BBOX":
@@ -88,6 +89,7 @@ class LayeredRFRender(torch.nn.Module):
         self.bkgd_use_space_time = bool(M.BKGD_USE_SPACE_TIME)
         self.use_deform_time = True
         self.scale, self.shift = scale, shift
+        self.rotation = rotation          # per layer: None, 3x3 matrix, rotation vector or (R, centre) (stnerf_b200.rotation)
         self.near, self.alpha = 0, 1
         self.precision = precision or getattr(M, "B200_PRECISION", "exact")
         self.chunk_rays = int(getattr(M, "B200_CHUNK_RAYS", 0))
@@ -252,6 +254,21 @@ class LayeredRFRender(torch.nn.Module):
         sc.shared_frame_id = 0 if self.retiming else 1
         return sc
 
+    def _rotation_entries(self):
+        """Every layer's parsed rotation (stnerf_b200.rotation.resolve): None or (R float32 (3,3), centre or None)."""
+        return ROT.resolve(self.rotation, self.layer_num + 1)
+
+    def _upload_rotation(self, nat) -> bytes:
+        """Set the model's rotation on the context (centres left to the library are each call's box centres).  Returns a key
+        that changes exactly when what was uploaded does."""
+        entries = self._rotation_entries()
+        if all(e is None for e in entries):
+            nat.set_rotation(None)
+            return b""
+        arrays = ROT.abi_arrays(entries)
+        nat.set_rotation(*arrays)
+        return b"".join(a.tobytes() for a in arrays)
+
     def _ensure_native(self, device):
         if self._native is None:
             with torch.cuda.device(device):
@@ -291,11 +308,12 @@ class LayeredRFRender(torch.nn.Module):
         if not self.retiming:
             frame_ids = frame_ids[:1].expand(l)                          # index_select(frame_id - 1) for every layer (:193)
         nat.set_scene(self._resolve_scene(frame_ids, density_threshold, bkgd_density_threshold))
+        self._upload_rotation(nat)                                       # after the scene: default centres are its boxes'
         if width == 7 and per_ray_frames:
             ids = rays[:, 6]
             if float(ids.min()) < 1 or float(ids.max()) >= self.bboxes.shape[0] + 1:
                 raise IndexError("frame id out of range for index_select(0, frame_id - 1) (layered_rfrender.py:193)")
-            key = (id(self.bboxes), repr(self.scale), repr(self.shift))
+            key = (id(self.bboxes), repr(self.scale), repr(self.shift), repr(self.rotation))
             if getattr(self, "_table_key", None) != key:
                 nat.set_box_table(self._box_table())
                 self._table_key = key
@@ -320,12 +338,12 @@ class LayeredRFRender(torch.nn.Module):
         return fine_mixed, coarse_mixed, fine_layer, coarse_layer, ray_mask
 
 
-def build_layered_model(cfg, camera_num=0, scale=None, shift=None):
+def build_layered_model(cfg, camera_num=0, scale=None, shift=None, rotation=None):
     """modeling/__init__.py:5-7.  cfg.MODEL.B200_TRAINABLE (default False) selects the trainable model
     (stnerf_b200.train.TrainableLayeredRFRender): network parameters, a differentiable forward whose networks train in
     cfg.MODEL.B200_TRAIN_PRECISION ("fp32", the default, or "tf32x3")."""
     if bool(getattr(cfg.MODEL, "B200_TRAINABLE", False)):
         from .train import TrainableLayeredRFRender
         return TrainableLayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift,
-                                        train_precision=getattr(cfg.MODEL, "B200_TRAIN_PRECISION", "fp32"))
-    return LayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift)
+                                        train_precision=getattr(cfg.MODEL, "B200_TRAIN_PRECISION", "fp32"), rotation=rotation)
+    return LayeredRFRender(cfg, camera_num=camera_num, scale=scale, shift=shift, rotation=rotation)

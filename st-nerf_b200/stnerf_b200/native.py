@@ -7,6 +7,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -48,6 +49,7 @@ class NativeRenderer:
         self._h = C.c_void_p()
         L.check(L.lib().stnerf_create(C.byref(self._h), C.byref(desc)), "stnerf_create")
         self._scene = None
+        self._rotation = None
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:
@@ -104,6 +106,23 @@ class NativeRenderer:
         t = table.detach().to("cpu", torch.float32).contiguous()
         assert t.dim() == 4 and tuple(t.shape[1:]) == (self.l, 2, 3), tuple(t.shape)
         L.check(L.lib().stnerf_set_box_table(self._h, L.ptr(t), int(t.shape[0])), "stnerf_set_box_table")
+
+    def set_rotation(self, modes=None, R=None, centres=None):
+        """Per-layer rotation (stnerf_set_rotation): modes (l,) of L.ROT_*, R (l,9) row-major, centres (l,3); modes=None
+        clears it.  Host-side only; skipped when unchanged."""
+        key = None if modes is None else tuple(np.ascontiguousarray(a).tobytes() for a in (modes, R, centres))
+        if key == self._rotation:
+            return
+        if modes is None:
+            L.check(L.lib().stnerf_set_rotation(self._h, None, None, None), "stnerf_set_rotation")
+        else:
+            m = np.ascontiguousarray(modes, dtype=np.int32)
+            r = np.ascontiguousarray(R, dtype=np.float32)
+            c = np.ascontiguousarray(centres, dtype=np.float32)
+            assert m.shape == (self.l,) and r.shape == (self.l, 9) and c.shape == (self.l, 3)
+            L.check(L.lib().stnerf_set_rotation(self._h, m.ctypes.data_as(C.c_void_p), r.ctypes.data_as(C.c_void_p),
+                                                c.ctypes.data_as(C.c_void_p)), "stnerf_set_rotation")
+        self._rotation = key
 
     # ---- render ----------------------------------------------------------------------------------------
     def render(self, rays: torch.Tensor, n1: int, n2: int, only_coarse: bool = False,
@@ -329,6 +348,21 @@ def marching_cubes(sigma: torch.Tensor, origin, step, level: float):
                                        L.stream_ptr()), "stnerf_mc_fill")
     del s, scratch
     return verts, faces
+
+
+def rotate_rays(rays: torch.Tensor, R, centre) -> torch.Tensor:
+    """A rotated layer's rays (stnerf_rotate_rays): columns 0..5 -> (c + R^T (o - c), R^T d), the rest copied.  rays (N, C)
+    contiguous fp32 CUDA; R (3,3), centre (3,)."""
+    r = _dev_f32(rays, "rays")
+    assert r.dim() == 2 and r.shape[1] >= 6
+    Rh = np.ascontiguousarray(np.asarray(R, dtype=np.float32).reshape(9))
+    ch = np.ascontiguousarray(np.asarray(centre, dtype=np.float32).reshape(3))
+    out = torch.empty_like(r)
+    with torch.cuda.device(r.device):
+        L.check(L.lib().stnerf_rotate_rays(L.ptr(r), r.shape[0], r.shape[1], Rh.ctypes.data_as(C.c_void_p),
+                                           ch.ctypes.data_as(C.c_void_p), L.ptr(out), L.stream_ptr()), "stnerf_rotate_rays")
+    del r
+    return out
 
 
 def launch_count() -> int:

@@ -29,6 +29,7 @@ class PoseRenderer:
         self.l = model.layer_num + 1
         self._svr: Optional[ShardedViewRenderer] = None
         self._pinned = None
+        self._rot_key = None          # the rotation the views made since the last native call were made with
 
     def _renderer(self) -> ShardedViewRenderer:
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -53,6 +54,12 @@ class PoseRenderer:
         ids = self.frame_ids(layer_frame_pair)
         self.model.retiming = True
         scene = self.model._resolve_scene(torch.tensor(ids), density_threshold, bkgd_density_threshold)
+        # the rotation lives on the context, not in the view: one native call renders every view with the same one (centres
+        # left to the library follow each view's boxes)
+        key = self.model._upload_rotation(svr.nat)
+        if self._rot_key is not None and key != self._rot_key:
+            raise ValueError("model.rotation changed between the views of one batch: a per-frame rotation needs batch=1")
+        self._rot_key = key
         self.model.seed += 1
         return svr.nat.make_view(K, pose, ids, scene, self.model.seed)
 
@@ -67,6 +74,7 @@ class PoseRenderer:
         """Several poses in ONE native call: (B, l+1, H, W, 5) on the device."""
         svr = self._renderer()
         views = []
+        self._rot_key = None
         for j in range(len(poses)):
             if per_frame_state is not None:
                 per_frame_state(first_index + j, self.model)
@@ -104,6 +112,7 @@ class PoseRenderer:
             if self.world == 1:
                 svr = self._renderer()
                 views = []
+                self._rot_key = None
                 for j in range(i0, i1):
                     if per_frame_state is not None:
                         per_frame_state(j, self.model)

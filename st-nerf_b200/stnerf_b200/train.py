@@ -76,8 +76,8 @@ class _ScatterFunction(torch.autograd.Function):
 class TrainableLayeredRFRender(LayeredRFRender):
     """LayeredRFRender with the reference's network submodules and a differentiable forward (module docstring)."""
 
-    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision=None, train_precision=None):
-        super().__init__(cfg, camera_num=camera_num, scale=scale, shift=shift, precision=precision)
+    def __init__(self, cfg, camera_num=0, scale=None, shift=None, precision=None, train_precision=None, rotation=None):
+        super().__init__(cfg, camera_num=camera_num, scale=scale, shift=shift, precision=precision, rotation=rotation)
         tp = train_precision or getattr(cfg.MODEL, "B200_TRAIN_PRECISION", "fp32")
         L.train_precision_code(tp)
         self.train_precision = tp
