@@ -153,7 +153,9 @@ int stnerf_rotate_rays(const float* rays, int64_t n, int ray_stride, const float
  *         a plane = rgb (n_rays,3) | depth (n_rays) | acc (n_rays)   (the tuples of :725-734).
  *         With only_coarse the fine planes are left untouched (the facade aliases them, :721-722).
  *         The caller's current device must be the one the context was created on (else STNERF_EINVAL).
- * ray_mask: (l, n_rays) uint8, |bin_width| > 1e-5 (layers/RaySamplePoint.py:105).                        */
+ * ray_mask: (l, n_rays) uint8, |bin_width| > 1e-5 (layers/RaySamplePoint.py:105).
+ * MotionNet's lerp (modeling/motion_net.py:53) is decided once per call: any hit ray of layer i with a fractional frame id,
+ * in any chunk, lerps layer i's time encoding for every ray of the call.                                 */
 int stnerf_render(stnerf_handle h, const float* rays, int64_t n_rays, int ray_stride, int n1, int n2,
                   int only_coarse, const float* jitter, const float* u, uint64_t seed,
                   float* out, uint8_t* ray_mask, void* stream);
@@ -241,9 +243,15 @@ int stnerf_composite_pass(const stnerf_scene* scene_host, int n_layers, int fine
 /* utils/dimension_kernel.py:24-33.  x (P,dim) -> out (P, dim*(1+2*n_freq)) */
 int stnerf_positional_encoding(const float* x, int64_t P, int dim, int n_freq, float* out, void* stream);
 /* modeling/spacenet.py:101-160.  pos (P,3), dirs (P,3), times (P)|NULL -> rgb (P,3) raw, sigma (P) raw.
+ * In STNERF_PREC_TC_3XF16_CF both passes' weights run with the correction products first.
  * Here and in stnerf_motionnet, P = 0 succeeds without reading or writing anything (the pointers may be NULL). */
 int stnerf_spacenet(stnerf_handle h, int layer, int fine, const float* pos, const float* dirs, const float* times,
                     int64_t P, float* rgb, float* sigma, void* stream);
+/* stnerf_spacenet in the weight-stage schedule stnerf_render uses for pass `fine`: the same call except in
+ * STNERF_PREC_TC_3XF16_CF, whose fine pass keeps the interleaved order (corrections first in the coarse pass only).  A render's
+ * SpaceNet outputs are this call's on the same points, bit for bit, in every precision.                                  */
+int stnerf_spacenet_pass(stnerf_handle h, int layer, int fine, const float* pos, const float* dirs, const float* times,
+                         int64_t P, float* rgb, float* sigma, void* stream);
 /* modeling/motion_net.py:34-71.  xyzt (P,4) -> flow (P,3).  lerp_mode: -1 = decide like the reference
  * (any non-integer t in the batch, :53), 0/1 = force.                                                      */
 int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
@@ -257,6 +265,8 @@ int stnerf_motionnet(stnerf_handle h, int layer, const float* xyzt, int64_t P, i
  *   2. a performer (layer >= 1): flow = MotionNet(p, frame_id) and p += flow, one round-to-nearest fp32 add (:340-356 /
  *      :495-510); the time encoding is lerped exactly when frame_id is fractional (modeling/motion_net.py:53 for one frame);
  *   3. SpaceNet(p, dir, frame_id) (:397-409 / :552-563): the time input is frame_id when the net consumes time.
+ * The networks run as stnerf_motionnet / stnerf_spacenet run them: in STNERF_PREC_TC_3XF16_CF the fine SpaceNet, too, adds
+ * its correction products first, where the render's fine pass interleaves them (stnerf_spacenet_pass).
  * Layer and weight errors return STNERF_EINVAL / STNERF_ENOWEIGHTS; a call before stnerf_set_scene returns STNERF_EINVAL.   */
 typedef struct {
   float origin[3];                               /* point (i,j,k) = origin + (i,j,k)*step: one fp32 product and one fp32 sum  */

@@ -520,7 +520,7 @@ static int run_spacenet(stnerf_ctx* c, const PointSrc& src, SpaceNetDev& net, fl
   if (src.mode == SRC_EXPLICIT) {      // unit entry point: one bias row per point, stream-ordered scratch
     float* cb = nullptr;
     STNERF_CUDA(cudaMallocAsync((void**)&cb, (size_t)std::max<long long>(src.n_slots, 1) * 128 * sizeof(float), st));
-    const int rc = tc_launch_spacenet(src, net.tc, c->precision, cb, raw, rgb, sigma, c->num_sms, st);
+    const int rc = tc_launch_spacenet(src, net.tc, c->precision, cb, raw, rgb, sigma, c->num_sms, st, nullptr, fine_pass);
     STNERF_CUDA(cudaFreeAsync(cb, st));
     return rc;
   }
@@ -624,7 +624,8 @@ struct ChunkHook {
 
 static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int ray_stride, int n1, int n2, int only_coarse,
                        const float* jitter, const float* u, uint64_t seed, OutSpec out, uint8_t* ray_mask, cudaStream_t st,
-                       const ChunkHook* before_chunk = nullptr, const ChunkHook* after_chunk = nullptr) {
+                       const ChunkHook* before_chunk = nullptr, const ChunkHook* after_chunk = nullptr,
+                       bool lerp_per_call = true) {
   if (!c || !rays || n_rays < 0) return STNERF_EINVAL;
   if (!c->have_scene) return STNERF_EINVAL;
   {                                         // the context's weights and workspace live on the device it was created on
@@ -645,13 +646,29 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
   RotatedRays rot;
   rc = rot.init(c, std::min(R, N), ray_stride, st);
   if (rc) return rc;
+  // MotionNet's lerp (motion_net.py:53) is decided once per call, over every hit ray of the call.  With more than one chunk, a
+  // sampling pass over all chunks sets the flags first (the chunk loop overwrites its depths, masks and hit lists).  Rays that
+  // share their frame-id columns (render_one_view) give every chunk the call's decision, so they skip it.
+  STNERF_CUDA(cudaMemsetAsync(c->lerp_flags, 0, STNERF_MAX_LAYERS * 4, st));
+  for (long long c0 = 0; lerp_per_call && N > R && c0 < N; c0 += R) {
+    const long long n = std::min(R, N - c0);
+    if (before_chunk) { rc = before_chunk->fn(before_chunk->user, c0, n, st); if (rc) return rc; }
+    const float* rch = rays + c0 * ray_stride;
+    STNERF_CUDA(cudaMemsetAsync(c->counts, 0, STNERF_MAX_LAYERS * 4, st));
+    LayerRays lr;
+    rc = rot.rotate(rch, n, lr);
+    if (rc) return rc;
+    rc = launch_sample(rch, n, ray_stride, c->dscene, l, n1, jitter ? jitter + c0 * n1 : nullptr, N * n1, seed, c0, c->idmap,
+                       c->t_coarse, R * c->cap_n1, c->mask_ws, R, c->hit, R, c->counts, c->lerp_flags, st, c->box_table,
+                       c->box_frames, &lr);
+    if (rc) return rc;
+  }
   for (long long c0 = 0; c0 < N; c0 += R) {
     const long long n = std::min(R, N - c0);
     if (before_chunk) { rc = before_chunk->fn(before_chunk->user, c0, n, st); if (rc) return rc; }
     c->last_chunk_rays = n; c->last_n1 = n1; c->last_s2 = n2 > 0 ? S2 : 0;
     const float* rch = rays + c0 * ray_stride;
     STNERF_CUDA(cudaMemsetAsync(c->counts, 0, STNERF_MAX_LAYERS * 4, st));
-    STNERF_CUDA(cudaMemsetAsync(c->lerp_flags, 0, STNERF_MAX_LAYERS * 4, st));
     uint8_t* mask = ray_mask ? ray_mask + c0 : c->mask_ws;
     const long long mask_ls = ray_mask ? N : R;
     int chunk_slot = -1;
@@ -875,7 +892,8 @@ static int render_one_view(stnerf_ctx* c, const stnerf_view* v, int H, int W, in
   const RayIdMap keep = c->idmap;
   c->idmap = RayIdMap{(long long)row0 * W, (long long)row_step * W, W};       // every pixel keeps the draws of an unsharded render
   OutSpec o{coarse_images, images, 1};
-  rc = render_core(c, c->v_rays, n, stride, n1, n2, 0, nullptr, nullptr, v->seed, o, nullptr, st);
+  rc = render_core(c, c->v_rays, n, stride, n1, n2, 0, nullptr, nullptr, v->seed, o, nullptr, st, nullptr, nullptr,
+                   /*lerp_per_call=*/false);
   c->idmap = keep;
   return rc;
 }
@@ -1099,8 +1117,9 @@ int stnerf_positional_encoding(const float* x, int64_t P, int dim, int n_freq, f
   return launch_posenc(x, P, dim, n_freq, out, (cudaStream_t)stream);
 }
 
-int stnerf_spacenet(stnerf_handle c, int layer, int fine, const float* pos, const float* dirs, const float* times,
-                    int64_t P, float* rgb, float* sigma, void* stream) {
+// One SpaceNet on explicit points; `render_schedule`: the weight-stage schedule the render's pass of these weights uses.
+static int spacenet_explicit(stnerf_ctx* c, int layer, int fine, const float* pos, const float* dirs, const float* times,
+                             int64_t P, float* rgb, float* sigma, cudaStream_t st, bool render_schedule) {
   if (!c || P < 0 || layer < 0 || layer >= c->l || (fine != 0 && fine != 1)) return STNERF_EINVAL;
   SpaceNetDev& net = c->space[fine][layer];
   if (!net.loaded) return STNERF_ENOWEIGHTS;
@@ -1110,7 +1129,17 @@ int stnerf_spacenet(stnerf_handle c, int layer, int fine, const float* pos, cons
   memset(&s, 0, sizeof(s));
   s.mode = SRC_EXPLICIT; s.pos = pos; s.dirs = dirs; s.times = times; s.pos_stride = 3; s.time_stride = 1;
   s.n_slots = P; s.S = 1; s.scale = 1.f;
-  return run_spacenet(c, s, net, nullptr, rgb, sigma, (cudaStream_t)stream);
+  return run_spacenet(c, s, net, nullptr, rgb, sigma, st, -1, nullptr, render_schedule && fine != 0);
+}
+
+int stnerf_spacenet(stnerf_handle c, int layer, int fine, const float* pos, const float* dirs, const float* times,
+                    int64_t P, float* rgb, float* sigma, void* stream) {
+  return spacenet_explicit(c, layer, fine, pos, dirs, times, P, rgb, sigma, (cudaStream_t)stream, false);
+}
+
+int stnerf_spacenet_pass(stnerf_handle c, int layer, int fine, const float* pos, const float* dirs, const float* times,
+                         int64_t P, float* rgb, float* sigma, void* stream) {
+  return spacenet_explicit(c, layer, fine, pos, dirs, times, P, rgb, sigma, (cudaStream_t)stream, true);
 }
 
 }  // extern "C"

@@ -94,6 +94,7 @@ _SIGNATURES = {
                                         C.c_int, _P, _P, _P, _P, _P]),
     "stnerf_positional_encoding": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
     "stnerf_spacenet": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P]),
+    "stnerf_spacenet_pass": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P, _P, _P]),
     "stnerf_motionnet": (C.c_int, [_P, C.c_int, _P, C.c_int64, C.c_int, _P, _P]),
     "stnerf_layer_field": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, _P, _P, C.c_int64, _P, _P, _P]),
     "stnerf_layer_grid": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, C.POINTER(Grid), _P, _P]),

@@ -218,7 +218,9 @@ class NativeRenderer:
         return out_host
 
     # ---- per-stage entry points that need the networks ------------------------------------------------------
-    def spacenet(self, layer: int, fine: bool, pos, dirs, times=None):
+    def spacenet(self, layer: int, fine: bool, pos, dirs, times=None, render_schedule: bool = False):
+        """rgb logits (P,3), raw sigma (P,1) of layer `layer`'s coarse / fine SpaceNet (stnerf_spacenet).  render_schedule: in the
+        weight-stage schedule the render uses for that pass (stnerf_spacenet_pass; differs only in exact_cf's fine pass)."""
         P = pos.shape[0]
         # the contiguous fp32 copies stay bound to locals until the call has been enqueued (a temporary would be
         # released -- and its block reused by the next .contiguous() -- before the kernel runs)
@@ -227,8 +229,9 @@ class NativeRenderer:
         rgb = torch.empty((P, 3), dtype=torch.float32, device=pos_c.device)
         sig = torch.empty((P, 1), dtype=torch.float32, device=pos_c.device)
         with torch.cuda.device(pos_c.device):
-            L.check(L.lib().stnerf_spacenet(self._h, layer, 1 if fine else 0, L.ptr(pos_c), L.ptr(dirs_c), L.ptr(times_c),
-                                            P, L.ptr(rgb), L.ptr(sig), L.stream_ptr()), "stnerf_spacenet")
+            fn = L.lib().stnerf_spacenet_pass if render_schedule else L.lib().stnerf_spacenet
+            L.check(fn(self._h, layer, 1 if fine else 0, L.ptr(pos_c), L.ptr(dirs_c), L.ptr(times_c), P, L.ptr(rgb), L.ptr(sig),
+                       L.stream_ptr()), "stnerf_spacenet")
         del pos_c, dirs_c, times_c
         return rgb, sig
 
