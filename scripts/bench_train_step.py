@@ -36,8 +36,8 @@ N_RAYS, N1, N2, LAYERS = 2000, 90, 30, 2
 MASK_SCALAR = 100000.0
 LR = 4e-4
 # the kernels of csrc/mlp_train.cu and mlp_train_tc.cu (SpaceNet / MotionNet training forward and backward)
-NETWORK_KERNELS = ("gemm_kernel", "tc_gemm_kernel", "reduce_partials_kernel", "rowsum_kernel", "spacenet_encode_kernel", "motionnet_encode_kernel",
-                   "spacenet_dpos_kernel")
+NETWORK_KERNELS = ("gemm_kernel", "tc_gemm_kernel", "reduce_partials_kernel", "rowsum_chunks_kernel", "rowsum_tree_kernel",
+                   "spacenet_encode_kernel", "motionnet_encode_kernel", "spacenet_dpos_kernel")
 
 
 def power_limit():

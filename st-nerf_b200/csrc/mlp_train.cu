@@ -11,8 +11,9 @@
 //   delta     d_in(k x P)    = W^T . d_out(n_out x P), masked by in > 0                  ("NT" in the points-major view)
 //   weights   dW(n_out x k)  = d_out . in^T, summed over points                          ("TN")
 // Weight and bias gradients are sums over the batch.  They are formed deterministically: the points are cut into chunks that
-// depend on P only, every CTA of a chunk writes its partial tile, and a second pass adds the partials in chunk order.  There
-// are no floating-point atomics, so two identical calls give identical bits.
+// depend on P only, every CTA of a chunk writes its partial tile, and a second pass adds the partials in chunk order (weights)
+// or in a fixed tree (biases, rowsum_chunks_kernel).  There are no floating-point atomics, so two identical calls give
+// identical bits.
 //
 // The forward GEMM starts every output at its bias and adds the k terms in ascending order with one fmaf each, exactly like
 // dense_layer in mlp_simt.cu, and the encodings use the same sincosf arguments: the training forward is bit-identical to
@@ -142,15 +143,32 @@ __global__ void reduce_partials_kernel(const float* __restrict__ part, int nz, l
   out[i] = s;
 }
 
-// out[m] = sum_p D(m, p): one CTA per row, a fixed thread-to-point assignment and a fixed tree
-__global__ void __launch_bounds__(TT) rowsum_kernel(Mat D, long long P, float* __restrict__ out) {
+// Bias gradients, out[m] = sum_p D(m, p), in two fixed trees: CTA (z, m) sums row m over point chunk z of grad_chunk(P) (each
+// thread at most chunk / TT points in sequence, then a tree over the threads) into part[z*M + m]; then one CTA per row adds
+// the chunk partials in a tree.  A single thread summing P / TT points in sequence (P = 2^20: 4096 fp32 adds) lost to
+// torch's own fp32 sum by 39x at P = 1 190 007; a run is now ceil(grad_chunk(P) / TT): 33 up to P = 1 081 344, 37 there.
+__global__ void __launch_bounds__(TT) rowsum_chunks_kernel(Mat D, long long P, long long chunk, float* __restrict__ part) {
   __shared__ float red[TT];
-  const int m = blockIdx.x, tid = threadIdx.x;
+  const int z = blockIdx.x, m = blockIdx.y, tid = threadIdx.x;
+  const long long pe = min(P, (z + 1) * chunk);
   float s = 0.f;
-  for (long long p = tid; p < P; p += TT) s += D.at(m, p);
+  for (long long p = z * chunk + tid; p < pe; p += TT) s += D.at(m, p);
   red[tid] = s;
   __syncthreads();
   for (int w = TT / 2; w > 0; w >>= 1) {
+    if (tid < w) red[tid] += red[tid + w];
+    __syncthreads();
+  }
+  if (tid == 0) part[(long long)z * gridDim.y + m] = red[0];
+}
+
+__global__ void __launch_bounds__(MAX_SPLIT) rowsum_tree_kernel(const float* __restrict__ part, int nz, int M,
+                                                                float* __restrict__ out) {
+  __shared__ float red[MAX_SPLIT];
+  const int m = blockIdx.x, tid = threadIdx.x;
+  red[tid] = tid < nz ? part[tid * M + m] : 0.f;
+  __syncthreads();
+  for (int w = MAX_SPLIT / 2; w > 0; w >>= 1) {
     if (tid < w) red[tid] += red[tid + w];
     __syncthreads();
   }
@@ -171,7 +189,12 @@ int weight_grad(Mat D, const float* h, int M, int N, long long P, float* dw, flo
   if (rc) return rc;
   reduce_partials_kernel<<<(unsigned)((MN + 255) / 256), 256, 0, st>>>(part, (int)nz, MN, dw);
   STNERF_LAUNCH_CHECK();
-  rowsum_kernel<<<M, TT, 0, st>>>(D, P, db);
+  // part is free again once the weight partials are reduced; nz <= MAX_SPLIT for every P (grad_chunk)
+  if (nz > 0) {
+    rowsum_chunks_kernel<<<dim3((unsigned)nz, (unsigned)M), TT, 0, st>>>(D, P, ch, part);
+    STNERF_LAUNCH_CHECK();
+  }
+  rowsum_tree_kernel<<<M, MAX_SPLIT, 0, st>>>(part, (int)nz, M, db);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
 }

@@ -50,8 +50,9 @@ MASK_SCALAR = 100000.0          # layered_trainer.py:244 `scalar_max`
 
 
 def case_inputs(name):
-    """fp32 rays, jitter (l,N,n1), u (l,N,n2) or None, labels (N,1) int64, target (N,3), state_dict."""
-    case = CASES[name]
+    """fp32 rays, jitter (l,N,n1), u (l,N,n2) or None, labels (N,1) int64, target (N,3), state_dict.  name: a key of CASES,
+    or a case dict of the same form."""
+    case = CASES[name] if isinstance(name, str) else name
     rays = C.rays_for(case)
     jit, u = C.uniforms_for(case)
     g = torch.Generator().manual_seed(700 + case["ray_seed"])

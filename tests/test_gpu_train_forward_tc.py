@@ -10,10 +10,8 @@ import torch
 
 import cases as C
 import test_gpu_composite_grad as CG
-import test_gpu_nets_train as NT
 import test_gpu_train_forward as TF
 import make_golden_train_grads as TG
-import train_restatement as TR
 from tests_support import make_cfg
 
 pytestmark = pytest.mark.gpu
@@ -43,60 +41,7 @@ def _model(case, train_precision="tf32x3", sd=None, set_knob=True):
 
 @pytest.mark.parametrize("name", list(TG.CASES))
 def test_gradients_against_float64_on_the_reference_cases(name):
-    torch.backends.cuda.matmul.allow_tf32 = False
-    case = TG.CASES[name]
-    rays, jit, u, labels, target, sd = TG.case_inputs(name)
-    only_coarse, l = bool(case.get("only_coarse", False)), case["L"] + 1
-    model = _model(case, sd=sd)
-    assert all(m.train_precision == "tf32x3" for m in model.modules() if hasattr(m, "train_precision"))
-    lab, tgt = labels.to(DEV), target.to(DEV)
-
-    def native(keep):
-        model.zero_grad(set_to_none=True)
-        rec = TF._native_trace(model, keep)
-        model.inject_uniforms(jit.to(DEV).contiguous(), None if u is None else u.to(DEV).contiguous())
-        out = model(rays.to(DEV), lab, None, only_coarse, density_threshold=case["thr"][0], bkgd_density_threshold=case["thr"][1])
-        TG.trainer_loss(out, lab, tgt, only_coarse, rays.shape[0]).backward()
-        model.trace = None
-        return TF._grads(model), rec
-
-    _, rec = native(None)
-    samples = (rec["t_coarse"], rec["mask"])
-    fine_t = None if only_coarse else [rec["t_fine.%d" % i] for i in range(l)]
-    sc = C.scene_for(case)
-
-    def restated(dtype, device, keep=None, flow_at=None, kinks=None):
-        p = {k: v.to(device, dtype).clone().requires_grad_(True) for k, v in sd.items()}
-        r = {}
-        out = TR.forward(p, sc, rays, case["n1"], case["n2"], jit, u, only_coarse, case["thr"][0], case["thr"][1],
-                         bool(case.get("seven")), dtype, device, samples=samples, fine_t=fine_t, keep=keep, flow_at=flow_at,
-                         kinks=kinks, record=r)
-        if kinks is not None:
-            return None, None
-        TG.trainer_loss(out, labels.to(device), target.to(device, dtype), only_coarse, rays.shape[0]).backward()
-        return {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in p.items()}, r["flows"]
-
-    keep = {}
-    with torch.no_grad():
-        restated(torch.float64, DEV, kinks=keep)
-    nat, rec = native(keep)
-    flows_nat = {k[5:]: v for k, v in rec.items() if k.startswith("flow.")}
-    cpu, flows_cpu = restated(torch.float32, "cpu", keep)
-    gpu, flows_gpu = restated(torch.float32, DEV, keep)
-    truths = [restated(torch.float64, DEV, keep, flow_at=f)[0] for f in (flows_nat, flows_cpu, flows_gpu)]
-    used = [k for k in truths[0] if float(truths[0][k].abs().max()) > 0]
-    assert used
-    for group, factor in (([k for k in used if not k.startswith("time_deform_nets")], FACTOR),
-                          ([k for k in used if k.startswith("time_deform_nets")], CHAINED_FACTOR)):
-        if not group:
-            continue
-        e_nat = NT.grad_errors({k: nat[k] for k in group}, {k: truths[0][k] for k in group})
-        e_cpu = NT.grad_errors({k: cpu[k] for k in group}, {k: truths[1][k] for k in group})
-        e_gpu = NT.grad_errors({k: gpu[k] for k in group}, {k: truths[2][k] for k in group})
-        NT.assert_within_twice(e_nat, CG.yardstick(e_cpu, e_gpu), "tf32x3 %s (%d tensors)" % (name, len(group)), factor)
-    for k in nat:
-        if k not in used:
-            assert float(nat[k].abs().max()) == 0.0, k
+    TF.float64_step_check(TG.CASES[name], TG.case_inputs(name), "tf32x3", FACTOR, CHAINED_FACTOR)
 
 
 def test_identical_calls_give_identical_gradients():

@@ -11,7 +11,7 @@ test_gpu_composite_grad.py's training chain):
             gradient reaches the weights (the rest are detached);
   flow_at   per performer call: evaluate the SpaceNet at xyz + flow_at[call] with the gradient through this run's own flow;
   kinks     a dict that receives, per network call, the points none of whose hidden pre-activations is near a ReLU kink;
-  record    a dict that receives the flows (per call) and the fine depths.
+  record    a dict that receives the flows and the SpaceNet outputs (per call) and the fine depths.
 """
 from __future__ import annotations
 
@@ -123,7 +123,7 @@ def forward(p, scene, rays, n1, n2, jitter, u, only_coarse, thr, bthr, shared_fr
     pivot = None if scene.get("pivot") is None else scene["pivot"].to(**dd)
     shown = scene.get("shown", [True] * l)
     near, alpha2, boarder = float(scene.get("near", 0.0)), float(scene.get("alpha", 1.0)), float(scene.get("boarder", 1e10))
-    flows = {}
+    flows, outputs = {}, {}
 
     def sub(prefix):
         return {k[len(prefix):]: v.to(**dd) for k, v in p.items() if k.startswith(prefix)}
@@ -171,6 +171,7 @@ def forward(p, scene, rays, n1, n2, jitter, u, only_coarse, thr, bthr, shared_fr
             if i > 0:
                 kinks["m" + key] = kinks[key]
         r, s = O.spacenet_forward(w, q, dirs, times)
+        outputs[key] = (r.detach(), s.detach())
         r, s = gate(r, key), gate(s, key)
         rgb = rgb.index_put((idx,), r.reshape(M, S, 3))
         sig = sig.index_put((idx,), s.reshape(M, S))
@@ -202,7 +203,7 @@ def forward(p, scene, rays, n1, n2, jitter, u, only_coarse, thr, bthr, shared_fr
     coarse_layer = [x[:3] for x in outs]
     coarse_mixed = CG.merged_ref(ts, rgbs, sigs, boarder, None)
     if record is not None:
-        record["flows"] = flows
+        record["flows"], record["outputs"] = flows, outputs
     if only_coarse:
         return coarse_mixed, coarse_mixed, coarse_layer, coarse_layer, masks
     # ---- fine pass (:453-606) -----------------------------------------------------------------------------------------------
