@@ -398,6 +398,36 @@ int stnerf_train_uniforms(stnerf_handle h, int64_t n, int n2, uint64_t seed, flo
 int stnerf_weights_export(stnerf_handle h, void* host_buf, size_t capacity, size_t* bytes_needed);
 int stnerf_weights_import(stnerf_handle h, const void* host_buf, size_t bytes);
 
+/* ---- training ray pool: data/datasets/ray_dataset.py:339-460 + utils/ray_sampling.py:75-240 ---------------------------
+ * A pool entry is 16 bytes (uint32 x4): pixel (row * W + col) | camera + frame slot << 16 | r, g, b, label bytes | layer.
+ *
+ * Selection of one (image, layer), replacing the per-camera ray_sampling_label_label (ray_sampling.py:194-240: keep
+ * label == layer) and ray_sampling_label_bbox (:75-175: keep the rows [r0,r1) x cols [c0,c1) of the box's projected
+ * rectangle).  `label` is a DEVICE map of H*W uint8 (label_is_float = 0) or fp32 (1) values, or NULL for the constant map
+ * `const_label` (frame_dataset.py:278-284).  Kept pixels are compacted in row-major order; no atomic decides the order.
+ * stnerf_td_select_count enqueues the per-tile counts and their scan into `scratch` (stnerf_td_select_scratch_ints(H, W)
+ * ints); scratch[scratch_ints - 1] is then the number of kept pixels.  stnerf_td_select_write (same arguments, same
+ * scratch, after the count) writes pool entries (rgb = DEVICE H*W*3 uint8, uint8 labels only) and/or the pixel indices.
+ * rect_host = {r0, r1, c0, c1} for STNERF_TD_BY_RECT.  Bad arguments return STNERF_EINVAL.                                */
+#define STNERF_TD_BY_LABEL 0
+#define STNERF_TD_BY_RECT 1
+int64_t stnerf_td_select_scratch_ints(int H, int W);
+int stnerf_td_select_count(const void* label, int label_is_float, int const_label, int H, int W, int mode, int layer,
+                           const int* rect_host, int* scratch, void* stream);
+int stnerf_td_select_write(const void* label, int label_is_float, int const_label, const uint8_t* rgb, int H, int W,
+                           int mode, int layer, const int* rect_host, int camera, int frame_slot, const int* scratch,
+                           void* pool, int* pixels, void* stream);
+/* One training batch from B pool indices (int32 or int64 `idx`, DEVICE), replacing Ray_Frame_Layer_Dataset.__getitem__
+ * (ray_dataset.py:459-460) + default collate: rays (B, 6 + time_col) by the same arithmetic as stnerf_raygen, with frame id
+ * frame_base + frame slot in column 6 when time_col = 1 (:416-418); rgbs (B,3) = byte / 255; labels, bbox_labels (B,1);
+ * bboxes (B,8,3); near_far (B,2).  Tables (DEVICE fp32): cams [n_geom][n_cams][24] = K^-1 (9) | R (9) | origin (3) | W | 2
+ * unused; boxes [n_layers][n_frames][24]; near_far [n_layers][n_frames][n_cams][2].  geom_of_layer_host[l] picks layer
+ * l's camera table.  Enqueues one kernel; no host sync, no allocation.                                                    */
+int stnerf_td_batch(const void* pool, const void* idx, int idx_is_64, int64_t B, const float* cams,
+                    const int* geom_of_layer_host, int n_layers, int n_cams, const float* boxes, const float* near_far,
+                    int n_frames, float frame_base, int time_col, float* rays, float* rgbs, float* labels,
+                    float* bbox_labels, float* bboxes, float* near_far_out, void* stream);
+
 /* Tensor-core plumbing self-test: one 128x256x64 fp16 product through the library's warpgroup-MMA descriptors, swizzled
  * layouts, bulk copy and accumulator fragment; writes max |D - host reference| (expected < 1e-3).                           */
 int stnerf_selftest_umma(float* max_err_host);

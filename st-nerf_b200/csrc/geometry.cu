@@ -4,6 +4,7 @@
 // (layers/RaySamplePoint.py:17-32,98-105), and several results feed discontinuous tests (inclusive face
 // tests, |bin_width| > 1e-5, t < 0), so products and sums must round separately exactly as eager PyTorch does.
 #include "common.cuh"
+#include "raygen.cuh"
 
 namespace stnerf {
 
@@ -268,18 +269,10 @@ __global__ void raygen_kernel(RayGenParams P, int W, int row0, int row_step, int
   if (idx >= total) return;
   const int rr = (int)(idx / W), j = (int)(idx - (long long)rr * W);
   const float px = (float)j, py = (float)(row0 + rr * row_step);
-  // dirs = K^-1 (col, row, 1)
   float c[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) c[a] = (P.kinv[3 * a] * px + P.kinv[3 * a + 1] * py) + P.kinv[3 * a + 2];
-  const float nrm = sqrtf((c[0] * c[0] + c[1] * c[1]) + c[2] * c[2]);
-  c[0] = c[0] / nrm; c[1] = c[1] / nrm; c[2] = c[2] / nrm;
+  raygen_dir(P.kinv, px, py, c);        // dirs = K^-1 (col, row, 1)
   float* out = rays + idx * ray_stride;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    out[a] = P.org[a];
-    out[3 + a] = (P.rot[3 * a] * c[0] + P.rot[3 * a + 1] * c[1]) + P.rot[3 * a + 2] * c[2];
-  }
+  raygen_write(P.rot, P.org, c, out);
   for (int f = 0; f < P.n_fid; ++f) out[6 + f] = P.fid[f];
 }
 

@@ -14,6 +14,9 @@ MAX_S = 512
 # stnerf_set_rotation modes: no rotation, about an explicit centre, about the centre of the layer's box in each call's scene
 ROT_OFF, ROT_CENTRE, ROT_BOX = 0, 1, 2
 
+# stnerf_td_select modes: keep label == layer, keep a box's projected rectangle
+TD_BY_LABEL, TD_BY_RECT = 0, 1
+
 PREC_FP32_SIMT, PREC_TC_3XF16, PREC_TC_F16, PREC_TC_MIXED, PREC_TC_3XF16_CF = 0, 1, 2, 3, 4
 PRECISIONS = {"fp32": PREC_FP32_SIMT, "exact": PREC_TC_3XF16, "tc3": PREC_TC_3XF16, "fast": PREC_TC_F16, "mixed": PREC_TC_MIXED,
               "exact_cf": PREC_TC_3XF16_CF}
@@ -119,6 +122,12 @@ _SIGNATURES = {
     "stnerf_train_scatter": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),
     "stnerf_train_gather": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P, _P, _P, _P, _P, _P]),
     "stnerf_train_uniforms": (C.c_int, [_P, C.c_int64, C.c_int, C.c_uint64, _P, _P]),
+    "stnerf_td_select_scratch_ints": (C.c_int64, [C.c_int, C.c_int]),
+    "stnerf_td_select_count": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "stnerf_td_select_write": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P,
+                                         _P, _P, _P]),
+    "stnerf_td_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, C.c_float, C.c_int,
+                                  _P, _P, _P, _P, _P, _P, _P]),
     "stnerf_debug_read_depths": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int64, C.c_int, _P]),
     "stnerf_launch_count": (C.c_uint64, []),
     "stnerf_set_ray_ids": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64]),

@@ -68,11 +68,19 @@ def ray_sampling(Ks, Ts, image_size, masks=None, mask_threshold=0.5, images=None
     return torch.cat(out, 0), None
 
 
-def ray_sampling_label_bbox(*a, **k):
-    raise NotImplementedError("training-time ray sampling is out of scope of the render hot path")
+def ray_sampling_label_bbox(image, label, K, T, bbox=None, bboxes=None):
+    """utils/ray_sampling.py:75-192: rays / labels / rgbs of the pixels in the box's projected rectangle (all pixels without
+    a box), the (H,W,1) ray mask, and with `bboxes` each ray's box by its label.  Pixels are chosen and rays generated on the
+    GPU; the results are returned on the input's device."""
+    from stnerf_b200 import train_data
+    return train_data.sample_label_bbox(image, label, K, T, bbox=bbox, bboxes=bboxes)
 
 
-ray_sampling_label_label = ray_sampling_label_bbox
+def ray_sampling_label_label(image, label, K, T, label0):
+    """utils/ray_sampling.py:194-240: rays / labels / rgbs of the pixels whose label is label0, and the (H,W,1) ray mask."""
+    from stnerf_b200 import train_data
+    return train_data.sample_label_label(image, label, K, T, label0)
+
 
 __all__ = ["Trigonometric_kernel", "sample_pdf", "generate_rays", "ray_sampling", "batchify_ray",
            "layered_batchify_ray", "layered_batchify_ray_big", "ray_sampling_label_bbox", "ray_sampling_label_label",
