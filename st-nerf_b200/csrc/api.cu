@@ -255,6 +255,25 @@ static size_t bind_motionnet(MotionNetDev& N) {
   return cur;
 }
 
+// Install a network's SIMT image and scalar biases on the context.  The caller adds the tensor-core weights, then marks it loaded.
+static int install_spacenet(SpaceNetDev& N, const std::vector<float>& simt, bool use_time, float b_sigma, const float* b_rgbo) {
+  N.loaded = false;
+  const int rc = upload(&N.blob, simt);
+  if (rc) return rc;
+  if (bind_spacenet(N, use_time) != simt.size()) return STNERF_EINVAL;
+  N.w.b_sigma = b_sigma;
+  for (int a = 0; a < 3; ++a) N.w.b_rgbo[a] = b_rgbo[a];
+  return STNERF_OK;
+}
+static int install_motionnet(MotionNetDev& N, const std::vector<float>& simt, const float* b_out) {
+  N.loaded = false;
+  const int rc = upload(&N.blob, simt);
+  if (rc) return rc;
+  if (bind_motionnet(N) != simt.size()) return STNERF_EINVAL;
+  for (int a = 0; a < 3; ++a) N.w.b_out[a] = b_out[a];
+  return STNERF_OK;
+}
+
 int stnerf_load_spacenet(stnerf_handle c, int layer, int fine, const float* blob, size_t n) {
   if (!c || !blob || layer < 0 || layer >= c->l || (fine != 0 && fine != 1)) return STNERF_EINVAL;
   const bool use_time = (n == (size_t)SPACENET_FLOATS_TIME);
@@ -276,14 +295,9 @@ int stnerf_load_spacenet(stnerf_handle c, int layer, int fine, const float* blob
   transpose_into(host, p, HEAD, krgb); p += (size_t)HEAD * krgb;
   host.insert(host.end(), p, p + HEAD); p += HEAD;
   host.insert(host.end(), p, p + 3 * HEAD); p += 3 * HEAD;
-  const float b_o[3] = {p[0], p[1], p[2]};
   SpaceNetDev& N = c->space[fine][layer];
-  N.loaded = false;
-  int rc = upload(&N.blob, host);
+  int rc = install_spacenet(N, host, use_time, b_sigma, p);
   if (rc) return rc;
-  if (bind_spacenet(N, use_time) != host.size()) return STNERF_EINVAL;
-  N.w.b_sigma = b_sigma;
-  for (int a = 0; a < 3; ++a) N.w.b_rgbo[a] = b_o[a];
   rc = tc_pack_spacenet(N.tc, blob, use_time);
   if (rc) return rc;
   N.loaded = true;
@@ -301,11 +315,8 @@ int stnerf_load_motionnet(stnerf_handle c, int layer, const float* blob, size_t 
   }
   host.insert(host.end(), p, p + 3 * HEAD); p += 3 * HEAD;
   MotionNetDev& N = c->motion[layer];
-  N.loaded = false;
-  int rc = upload(&N.blob, host);
+  int rc = install_motionnet(N, host, p);
   if (rc) return rc;
-  if (bind_motionnet(N) != host.size()) return STNERF_EINVAL;
-  for (int a = 0; a < 3; ++a) N.w.b_out[a] = p[a];
   rc = tc_pack_motionnet(N.tc, blob);
   if (rc) return rc;
   N.loaded = true;
@@ -408,22 +419,15 @@ int stnerf_weights_import(stnerf_handle c, const void* buf, size_t bytes) {
     const std::vector<float> host(simt, simt + r.simt_floats);
     if (r.kind == 0) {
       SpaceNetDev& N = c->space[r.fine][r.layer];
-      N.loaded = false;
-      int rc = upload(&N.blob, host);
+      int rc = install_spacenet(N, host, r.use_time != 0, r.scalars[0], r.scalars + 1);
       if (rc) return rc;
-      bind_spacenet(N, r.use_time != 0);
-      N.w.b_sigma = r.scalars[0];
-      for (int a = 0; a < 3; ++a) N.w.b_rgbo[a] = r.scalars[1 + a];
       rc = tc_import(N.tc, true, (int)r.use_time, stream, aux, tail);
       if (rc) return rc;
       N.loaded = true;
     } else {
       MotionNetDev& N = c->motion[r.layer];
-      N.loaded = false;
-      int rc = upload(&N.blob, host);
+      int rc = install_motionnet(N, host, r.scalars);
       if (rc) return rc;
-      bind_motionnet(N);
-      for (int a = 0; a < 3; ++a) N.w.b_out[a] = r.scalars[a];
       rc = tc_import(N.tc, false, 0, stream, aux, nullptr);
       if (rc) return rc;
       N.loaded = true;
@@ -503,12 +507,47 @@ struct RotatedRays {
 // ---------------------------------------------------------------------------------------------------------
 // one pass of the networks over a chunk
 // ---------------------------------------------------------------------------------------------------------
-static void fill_edit(PointSrc& s, const stnerf_scene& sc, int layer, bool fine) {
-  s.shift_on = sc.shift_on[layer];
-  s.scale_on = fine ? sc.scale_fine_on[layer] : sc.scale_coarse_on[layer];
-  for (int a = 0; a < 3; ++a) { s.shift[a] = sc.shift[layer][a]; s.pivot[a] = sc.pivot[a]; }
-  s.scale = sc.scale[layer];
-  if (!s.scale_on) s.scale = 1.0f;
+// The inverse edit of one layer and pass (common.cuh: inverse_edit) into a PointSrc or a FieldEdit.
+template <class E>
+static void fill_edit(E& e, const stnerf_scene& sc, int layer, bool fine) {
+  e.shift_on = sc.shift_on[layer];
+  e.scale_on = fine ? sc.scale_fine_on[layer] : sc.scale_coarse_on[layer];
+  for (int a = 0; a < 3; ++a) { e.shift[a] = sc.shift[layer][a]; e.pivot[a] = sc.pivot[a]; }
+  e.scale = e.scale_on ? sc.scale[layer] : 1.0f;
+}
+
+// n points given one by one: pos (n, pos_stride), dirs (n,3) or null, times (n, time_stride) or null.
+static PointSrc explicit_src(const float* pos, int pos_stride, const float* dirs, const float* times, int time_stride, long long n) {
+  PointSrc s;
+  memset(&s, 0, sizeof(s));
+  s.mode = SRC_EXPLICIT; s.pos = pos; s.pos_stride = pos_stride; s.dirs = dirs; s.times = times; s.time_stride = time_stride;
+  s.n_slots = n; s.S = 1; s.scale = 1.f;
+  return s;
+}
+
+// Layer `layer`'s samples at depths t (ray, S) along `rays`, with the inverse edit of the pass; the caller adds which rays
+// (hit, count, slots).
+static PointSrc march_src(const stnerf_ctx* c, int layer, bool fine, const float* rays, int ray_stride, const float* t, int S) {
+  PointSrc s;
+  memset(&s, 0, sizeof(s));
+  s.mode = SRC_MARCH;
+  s.rays = rays; s.ray_stride = ray_stride; s.t = t; s.S = S;
+  s.layer = c->scene.shared_frame_id ? 0 : layer;             // frame-id column offset of this layer
+  fill_edit(s, c->scene, layer, fine);
+  return s;
+}
+
+// The context has a scene (unless the call reads none) and is on its own device, where its weights and workspace live.
+static int ctx_ready(const stnerf_ctx* c, bool need_scene = true) {
+  if (need_scene && !c->have_scene) return STNERF_EINVAL;
+  int cur = -1;
+  STNERF_CUDA(cudaGetDevice(&cur));
+  return cur == c->device ? STNERF_OK : STNERF_EINVAL;
+}
+
+// Rays carry o, d and a frame-id column per layer, or one shared column (the reference prints + exit(-1) otherwise, :162-163).
+static bool ray_stride_ok(const stnerf_ctx* c, int ray_stride) {
+  return ray_stride >= 6 + (c->scene.shared_frame_id ? 1 : c->l);
 }
 
 static int run_spacenet(stnerf_ctx* c, const PointSrc& src, SpaceNetDev& net, float* raw, float* rgb, float* sigma,
@@ -548,14 +587,7 @@ static int run_nets(stnerf_ctx* c, const LayerRays& rays, long long n, int ray_s
   const long long tl = R * (fine ? c->cap_s2 : c->cap_n1);      // layer strides of the workspace arrays
   for (int i = 0; i < c->l; ++i) {
     if (i > 0 && !c->scene.shown[i]) continue;                  // hidden performers: sigma = rgb = 0 (:401, :556)
-    PointSrc s;
-    memset(&s, 0, sizeof(s));
-    s.mode = SRC_MARCH;
-    s.rays = rays.p[i]; s.ray_stride = ray_stride;                // a rotated layer marches along its own rays
-    s.t = tbuf + i * tl;
-    s.S = S; s.layer = c->scene.shared_frame_id ? 0 : i;      // frame-id column offset of this layer
-    s.pos_stride = 3; s.time_stride = 1;
-    fill_edit(s, c->scene, i, fine);
+    PointSrc s = march_src(c, i, fine, rays.p[i], ray_stride, tbuf + i * tl, S);   // a rotated layer marches along its own rays
     float* raw = want_raw ? rawbuf + (size_t)i * tl * 4 : nullptr;
     FuseCoarse f;
     memset(&f, 0, sizeof(f));
@@ -627,25 +659,31 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
                        const ChunkHook* before_chunk = nullptr, const ChunkHook* after_chunk = nullptr,
                        bool lerp_per_call = true) {
   if (!c || !rays || n_rays < 0) return STNERF_EINVAL;
-  if (!c->have_scene) return STNERF_EINVAL;
-  {                                         // the context's weights and workspace live on the device it was created on
-    int cur = -1;
-    STNERF_CUDA(cudaGetDevice(&cur));
-    if (cur != c->device) return STNERF_EINVAL;
-  }
-  if (ray_stride < 6 + (c->scene.shared_frame_id ? 1 : c->l)) return STNERF_EINVAL;   // the reference prints + exit(-1) (:162-163)
+  int rc = ctx_ready(c);
+  if (rc) return rc;
+  if (!ray_stride_ok(c, ray_stride)) return STNERF_EINVAL;
   if (n1 < 3 || n1 > STNERF_MAX_N1) return STNERF_EINVAL;
   if (only_coarse) n2 = 0;
   if (n2 < 0 || n1 + n2 > STNERF_MAX_S) return STNERF_EINVAL;
   if (n2 == 0 && !out.coarse) return STNERF_EINVAL;
   if (n2 > 0 && !out.fine) return STNERF_EINVAL;
-  int rc = ensure_ws(c, n1, n1 + n2);
+  rc = ensure_ws(c, n1, n1 + n2);
   if (rc) return rc;
   const int l = c->l, S2 = n1 + n2;
   const long long R = c->chunk_rays, N = n_rays;
   RotatedRays rot;
   rc = rot.init(c, std::min(R, N), ray_stride, st);
   if (rc) return rc;
+  // the coarse sampling of rays [c0, c0 + n): depths, masks, hit lists, counts and lerp flags; lr = where each layer's rays are
+  LayerRays lr;
+  auto sample = [&](long long c0, long long n, uint8_t* mask, long long mask_ls) -> int {
+    const float* rch = rays + c0 * ray_stride;
+    const int rc = rot.rotate(rch, n, lr);
+    if (rc) return rc;
+    return launch_sample(rch, n, ray_stride, c->dscene, l, n1, jitter ? jitter + c0 * n1 : nullptr, N * n1, seed, c0, c->idmap,
+                         c->t_coarse, R * c->cap_n1, mask, mask_ls, c->hit, R, c->counts, c->lerp_flags, st, c->box_table,
+                         c->box_frames, &lr);
+  };
   // MotionNet's lerp (motion_net.py:53) is decided once per call, over every hit ray of the call.  With more than one chunk, a
   // sampling pass over all chunks sets the flags first (the chunk loop overwrites its depths, masks and hit lists).  Rays that
   // share their frame-id columns (render_one_view) give every chunk the call's decision, so they skip it.
@@ -653,33 +691,21 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
   for (long long c0 = 0; lerp_per_call && N > R && c0 < N; c0 += R) {
     const long long n = std::min(R, N - c0);
     if (before_chunk) { rc = before_chunk->fn(before_chunk->user, c0, n, st); if (rc) return rc; }
-    const float* rch = rays + c0 * ray_stride;
     STNERF_CUDA(cudaMemsetAsync(c->counts, 0, STNERF_MAX_LAYERS * 4, st));
-    LayerRays lr;
-    rc = rot.rotate(rch, n, lr);
-    if (rc) return rc;
-    rc = launch_sample(rch, n, ray_stride, c->dscene, l, n1, jitter ? jitter + c0 * n1 : nullptr, N * n1, seed, c0, c->idmap,
-                       c->t_coarse, R * c->cap_n1, c->mask_ws, R, c->hit, R, c->counts, c->lerp_flags, st, c->box_table,
-                       c->box_frames, &lr);
+    rc = sample(c0, n, c->mask_ws, R);
     if (rc) return rc;
   }
   for (long long c0 = 0; c0 < N; c0 += R) {
     const long long n = std::min(R, N - c0);
     if (before_chunk) { rc = before_chunk->fn(before_chunk->user, c0, n, st); if (rc) return rc; }
     c->last_chunk_rays = n; c->last_n1 = n1; c->last_s2 = n2 > 0 ? S2 : 0;
-    const float* rch = rays + c0 * ray_stride;
     STNERF_CUDA(cudaMemsetAsync(c->counts, 0, STNERF_MAX_LAYERS * 4, st));
     uint8_t* mask = ray_mask ? ray_mask + c0 : c->mask_ws;
     const long long mask_ls = ray_mask ? N : R;
     int chunk_slot = -1;
-    LayerRays lr;
     {
       ProfScope ps(c, 2, (double)n, -1, 1, st);
-      rc = rot.rotate(rch, n, lr);
-      if (rc) return rc;
-      rc = launch_sample(rch, n, ray_stride, c->dscene, l, n1, jitter ? jitter + c0 * n1 : nullptr, N * n1, seed, c0, c->idmap,
-                         c->t_coarse, R * c->cap_n1, mask, mask_ls, c->hit, R, c->counts, c->lerp_flags, st, c->box_table, c->box_frames,
-                         &lr);
+      rc = sample(c0, n, mask, mask_ls);
       if (rc) return rc;
     }
     if (c->prof_on && c->prof_counts && c->prof_chunks < PROF_MAX_CHUNKS) {
@@ -1125,11 +1151,8 @@ static int spacenet_explicit(stnerf_ctx* c, int layer, int fine, const float* po
   if (!net.loaded) return STNERF_ENOWEIGHTS;
   if (P == 0) return STNERF_OK;        // an empty batch has no buffers (an empty torch tensor's data pointer is null)
   if (!pos || !dirs || !rgb || !sigma || (net.w.use_time && !times)) return STNERF_EINVAL;
-  PointSrc s;
-  memset(&s, 0, sizeof(s));
-  s.mode = SRC_EXPLICIT; s.pos = pos; s.dirs = dirs; s.times = times; s.pos_stride = 3; s.time_stride = 1;
-  s.n_slots = P; s.S = 1; s.scale = 1.f;
-  return run_spacenet(c, s, net, nullptr, rgb, sigma, st, -1, nullptr, render_schedule && fine != 0);
+  return run_spacenet(c, explicit_src(pos, 3, dirs, times, 1, P), net, nullptr, rgb, sigma, st, -1, nullptr,
+                      render_schedule && fine != 0);
 }
 
 int stnerf_spacenet(stnerf_handle c, int layer, int fine, const float* pos, const float* dirs, const float* times,
@@ -1152,6 +1175,14 @@ __global__ void any_fraction_kernel(const float* __restrict__ xyzt, long long P,
   }
 }
 
+// *flag = 1 when any of the P points (x, y, z, t) has a fractional t: MotionNet's lerp decision for a batch (motion_net.py:53)
+static int launch_any_fraction(const float* xyzt, long long P, int* flag, cudaStream_t st) {
+  STNERF_CUDA(cudaMemsetAsync(flag, 0, 4, st));
+  any_fraction_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(xyzt, P, flag);
+  STNERF_LAUNCH_CHECK();
+  return STNERF_OK;
+}
+
 extern "C" int stnerf_motionnet(stnerf_handle c, int layer, const float* xyzt, int64_t P, int lerp_mode, float* flow,
                                 void* stream) {
   if (!c || P < 0 || layer < 1 || layer >= c->l || lerp_mode < -1 || lerp_mode > 1) return STNERF_EINVAL;
@@ -1161,15 +1192,10 @@ extern "C" int stnerf_motionnet(stnerf_handle c, int layer, const float* xyzt, i
   if (!xyzt || !flow) return STNERF_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
   if (lerp_mode < 0) {
-    STNERF_CUDA(cudaMemsetAsync(c->any_frac, 0, 4, st));
-    any_fraction_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(xyzt, P, c->any_frac);
-    STNERF_LAUNCH_CHECK();
+    const int rc = launch_any_fraction(xyzt, P, c->any_frac, st);
+    if (rc) return rc;
   }
-  PointSrc s;
-  memset(&s, 0, sizeof(s));
-  s.mode = SRC_EXPLICIT; s.pos = xyzt; s.times = xyzt + 3; s.pos_stride = 4; s.time_stride = 4;
-  s.n_slots = P; s.S = 1; s.scale = 1.f;
-  return run_motionnet(c, s, net, c->any_frac, lerp_mode, nullptr, flow, st);
+  return run_motionnet(c, explicit_src(xyzt, 4, nullptr, xyzt + 3, 4, P), net, c->any_frac, lerp_mode, nullptr, flow, st);
 }
 
 // ---- a layer's field at one frame (extract.cu builds the points; the networks are the render's) ------------------------------
@@ -1178,22 +1204,15 @@ static constexpr long long FIELD_CHUNK = 1LL << 20;
 static int field_check(stnerf_ctx* c, int layer, int fine, float frame_id) {
   if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || !isfinite(frame_id)) return STNERF_EINVAL;
   if (!c->space[fine][layer].loaded || (layer > 0 && !c->motion[layer].loaded)) return STNERF_ENOWEIGHTS;
-  if (!c->have_scene) return STNERF_EINVAL;
-  int cur = -1;                                       // the context's scene and weights live on the device it was created on
-  STNERF_CUDA(cudaGetDevice(&cur));
-  return cur == c->device ? STNERF_OK : STNERF_EINVAL;
+  return ctx_ready(c);
 }
 
 // Points [0, P) of `xyz` (or of grid `g` when xyz == null) through the edit, the MotionNet and the SpaceNet, chunk by chunk.
 static int field_run(stnerf_ctx* c, int layer, int fine, float frame_id, const float* xyz, const FieldGrid& g, long long P,
                      const float* dirs, float* rgb, float* sigma, cudaStream_t st) {
-  const stnerf_scene& sc = c->scene;
   FieldEdit e;
   memset(&e, 0, sizeof(e));
-  e.shift_on = sc.shift_on[layer];
-  e.scale_on = fine ? sc.scale_fine_on[layer] : sc.scale_coarse_on[layer];
-  for (int a = 0; a < 3; ++a) { e.shift[a] = sc.shift[layer][a]; e.pivot[a] = sc.pivot[a]; }
-  e.scale = e.scale_on ? sc.scale[layer] : 1.0f;
+  fill_edit(e, c->scene, layer, fine != 0);
   e.rot_on = layer_rot(c, layer, false, e.rot) ? 1 : 0;
   const bool rot_dirs = e.rot_on && dirs;                             // the SpaceNet looks along R^T dir
   const int lerp = floorf(frame_id) != frame_id ? 1 : 0;              // motion_net.py:53 for a batch of one frame
@@ -1208,21 +1227,11 @@ static int field_run(stnerf_ctx* c, int layer, int fine, float frame_id, const f
   for (long long p0 = 0; p0 < P && !rc; p0 += chunk) {
     const long long n = std::min(chunk, P - p0);
     rc = launch_field_points(xyz, g, p0, n, e, frame_id, xyzt, dirs, rdirs, st);
-    if (!rc && layer > 0) {                                            // :340-356 / :495-510: xyz += MotionNet(xyz, t)
-      PointSrc m;
-      memset(&m, 0, sizeof(m));
-      m.mode = SRC_EXPLICIT; m.pos = xyzt; m.times = xyzt + 3; m.pos_stride = 4; m.time_stride = 4;
-      m.n_slots = n; m.S = 1; m.scale = 1.f;
-      rc = run_motionnet(c, m, c->motion[layer], nullptr, lerp, def, nullptr, st);
-    }
+    if (!rc && layer > 0)                                              // :340-356 / :495-510: xyz += MotionNet(xyz, t)
+      rc = run_motionnet(c, explicit_src(xyzt, 4, nullptr, xyzt + 3, 4, n), c->motion[layer], nullptr, lerp, def, nullptr, st);
     if (rc) break;
-    PointSrc s;
-    memset(&s, 0, sizeof(s));
-    s.mode = SRC_EXPLICIT;
-    s.pos = layer > 0 ? def : xyzt; s.pos_stride = layer > 0 ? 3 : 4;
-    s.dirs = rot_dirs ? rdirs : dirs ? dirs + 3 * p0 : zdirs;
-    s.times = xyzt + 3; s.time_stride = 4;
-    s.n_slots = n; s.S = 1; s.scale = 1.f;
+    const PointSrc s = explicit_src(layer > 0 ? def : xyzt, layer > 0 ? 3 : 4, rot_dirs ? rdirs : dirs ? dirs + 3 * p0 : zdirs,
+                                    xyzt + 3, 4, n);
     rc = run_spacenet(c, s, c->space[fine][layer], nullptr, rgb ? rgb + 3 * p0 : nullptr, sigma + p0, st);
   }
   if (cudaFreeAsync(buf, st) != cudaSuccess && !rc) rc = STNERF_ECUDA;
@@ -1320,9 +1329,8 @@ int stnerf_motionnet_train_forward_prec(const float* weights, const float* xyzt,
   cudaStream_t st = (cudaStream_t)stream;
   int* flag = (int*)scratch;
   if (lerp_mode < 0) {
-    STNERF_CUDA(cudaMemsetAsync(flag, 0, 4, st));
-    any_fraction_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(xyzt, P, flag);
-    STNERF_LAUNCH_CHECK();
+    const int rc = launch_any_fraction(xyzt, P, flag, st);
+    if (rc) return rc;
   }
   return launch_motionnet_train_forward(weights, xyzt, P, flag, lerp_mode, flow, saved, st, precision);
 }
@@ -1362,26 +1370,13 @@ int stnerf_composite_backward(const float* t, const float* rgb, const float* sig
 }
 
 // ---- training: the per-sample work around the networks (train_march.cu) ------------------------------------------------------
-static int on_ctx_device(stnerf_ctx* c) {          // the context's scene and weights live on the device it was created on
-  int cur = -1;
-  STNERF_CUDA(cudaGetDevice(&cur));
-  return cur == c->device ? STNERF_OK : STNERF_EINVAL;
-}
-
-static int train_ready(stnerf_ctx* c, int ray_stride) {
-  if (!c->have_scene) return STNERF_EINVAL;
-  int rc = on_ctx_device(c);
-  if (rc) return rc;
-  if (ray_stride < 6 + (c->scene.shared_frame_id ? 1 : c->l)) return STNERF_EINVAL;
-  return STNERF_OK;
-}
-
 int stnerf_train_sample(stnerf_handle c, const float* rays, int64_t n, int ray_stride, int n1, const float* jitter, uint64_t seed,
                         float* t, uint8_t* mask, int32_t* hit, int32_t* hit_counts_host, int32_t* any_frac_host, void* stream) {
   if (!c || n < 0 || n1 < 3 || n1 > STNERF_MAX_N1 || !hit_counts_host || !any_frac_host) return STNERF_EINVAL;
   if ((long long)n * STNERF_MAX_S >= (1LL << 31)) return STNERF_EINVAL;      // 32-bit sample indices, as for a render chunk
-  int rc = train_ready(c, ray_stride);
+  int rc = ctx_ready(c);
   if (rc) return rc;
+  if (!ray_stride_ok(c, ray_stride)) return STNERF_EINVAL;
   hit_counts_host[0] = (int32_t)n;
   any_frac_host[0] = 0;
   for (int i = 1; i < c->l; ++i) hit_counts_host[i] = any_frac_host[i] = 0;
@@ -1420,30 +1415,27 @@ int stnerf_train_points(stnerf_handle c, int layer, int fine, const float* rays,
                         const int32_t* hit, int64_t m, float* pos, float* dirs, float* times, float* xyzt, void* stream) {
   if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || n < 0 || m < 0 || S < 1 || S > STNERF_MAX_S) return STNERF_EINVAL;
   if ((layer == 0) != (hit == nullptr) || m > n || (layer == 0 && m != n)) return STNERF_EINVAL;
-  int rc = train_ready(c, ray_stride);
+  int rc = ctx_ready(c);
   if (rc) return rc;
+  if (!ray_stride_ok(c, ray_stride)) return STNERF_EINVAL;
   if (m == 0) return STNERF_OK;
   if (!rays || !t || (!pos && !dirs && !times && !xyzt)) return STNERF_EINVAL;
-  PointSrc s;
-  memset(&s, 0, sizeof(s));
-  s.mode = SRC_MARCH; s.rays = rays; s.ray_stride = ray_stride; s.t = t; s.S = S; s.hit = hit; s.n_slots = m;
-  s.layer = c->scene.shared_frame_id ? 0 : layer;
-  fill_edit(s, c->scene, layer, fine != 0);
   // a rotated layer: the points and directions of its own rays, as render_core marches them
   RotatedRays rot;
   rc = rot.init(c, n, ray_stride, (cudaStream_t)stream, layer);
   LayerRays lr;
   if (!rc) rc = rot.rotate(rays, n, lr);
   if (rc) return rc;
-  s.rays = lr.p[layer];
+  PointSrc s = march_src(c, layer, fine != 0, lr.p[layer], ray_stride, t, S);
+  s.hit = hit; s.n_slots = m;
   return launch_train_points(s, (long long)m * S, pos, dirs, times, xyzt, (cudaStream_t)stream);
 }
 
 int stnerf_train_scatter(stnerf_handle c, int layer, int fine, const float* t, int64_t n, int S, const int32_t* hit, int64_t m,
                          const float* rgb_c, const float* sigma_c, float* rgb, float* sigma, float* factor, void* stream) {
   if (!c || layer < 0 || layer >= c->l || (fine != 0 && fine != 1) || n < 0 || m < 0 || m > n || S < 1) return STNERF_EINVAL;
-  if ((layer == 0) != (hit == nullptr) || (layer == 0 && m != n) || !c->have_scene) return STNERF_EINVAL;
-  const int rc = on_ctx_device(c);
+  if ((layer == 0) != (hit == nullptr) || (layer == 0 && m != n)) return STNERF_EINVAL;
+  const int rc = ctx_ready(c);
   if (rc) return rc;
   if (n == 0) return STNERF_OK;
   if (!t || !rgb || !sigma || (m > 0 && (!rgb_c || !sigma_c || !factor))) return STNERF_EINVAL;
@@ -1453,7 +1445,7 @@ int stnerf_train_scatter(stnerf_handle c, int layer, int fine, const float* t, i
 int stnerf_train_gather(stnerf_handle c, int S, const int32_t* hit, int64_t m, const float* factor, const float* d_rgb,
                         const float* d_sigma, float* d_rgb_c, float* d_sigma_c, void* stream) {
   if (!c || m < 0 || S < 1) return STNERF_EINVAL;
-  const int rc = on_ctx_device(c);
+  const int rc = ctx_ready(c, /*need_scene=*/false);
   if (rc) return rc;
   if (m == 0) return STNERF_OK;
   if (!factor || !d_rgb_c || !d_sigma_c) return STNERF_EINVAL;

@@ -92,19 +92,26 @@ struct PointSrc {
   float shift[3], scale, pivot[3];
 };
 
+// The inverse edit of one layer and pass on a point (layered_rfrender.py:293-303 / :467-475), every op rounded on its own.
+// E is PointSrc or FieldEdit: any struct with the flat fields shift_on, scale_on, shift[3], scale, pivot[3].
+template <class E>
+__device__ __forceinline__ void inverse_edit(const E& e, float v[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if (e.shift_on) v[a] = __fsub_rn(v[a], e.shift[a]);                                        // :298 / :471
+    if (e.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], e.pivot[a]), e.scale), e.pivot[a]);   // :303 / :475
+  }
+}
+
 // A marched sample p = t*d + o with separately rounded product and sum (layers/RaySamplePoint.py:103,
-// layered_rfrender.py:465), then the inverse edit of the pass (:293-303 / :467-475).  rp = the ray (o at 0..2), d = its
-// direction.  Shared by the SIMT networks' SRC_MARCH fetch and the training point assembly, so both round alike.
+// layered_rfrender.py:465), then the inverse edit of the pass.  rp = the ray (o at 0..2), d = its direction.  Shared by both
+// networks' SRC_MARCH fetch and the training point assembly, so all of them round alike.
 __device__ __forceinline__ void march_point(const PointSrc& s, const float* rp, float tt, float dx, float dy, float dz,
                                             float v[3]) {
   v[0] = __fadd_rn(__fmul_rn(tt, dx), rp[0]);
   v[1] = __fadd_rn(__fmul_rn(tt, dy), rp[1]);
   v[2] = __fadd_rn(__fmul_rn(tt, dz), rp[2]);
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    if (s.shift_on) v[a] = __fsub_rn(v[a], s.shift[a]);                                        // :298 / :471
-    if (s.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], s.pivot[a]), s.scale), s.pivot[a]);   // :303 / :475
-  }
+  inverse_edit(s, v);
 }
 
 __device__ __forceinline__ long long src_num_points(const PointSrc& s) {
@@ -277,7 +284,7 @@ struct FieldGrid {           // point (i,j,k) = origin + (i,j,k)*step, one produ
   float origin[3], step[3];
   int dims[3];
 };
-struct FieldEdit {           // the inverse edit of one layer and pass (the edit part of march_point), rotation first
+struct FieldEdit {           // the inverse edit of one layer and pass (inverse_edit), rotation first
   int shift_on, scale_on, rot_on;
   float shift[3], scale, pivot[3];
   RayRot rot;

@@ -1,7 +1,7 @@
 // Geometry extraction: the points of a layer's density field at one frame, and marching cubes on a sampled grid.
 //
 // field_points_kernel builds the network inputs of stnerf_layer_field / stnerf_layer_grid: a world point (given, or grid point
-// origin + (i,j,k)*step), the inverse edit of the pass with the rounding of march_point (common.cuh), and the frame id as the
+// origin + (i,j,k)*step), the inverse edit of the pass (inverse_edit, common.cuh), and the frame id as the
 // time column.  api.cu then runs the context's MotionNet / SpaceNet on them (SRC_EXPLICIT), as stnerf_render does.
 //
 // Marching cubes (no context): a corner is inside when v > level (NaN is outside).  Every grid point owns the vertices of its
@@ -49,12 +49,7 @@ field_points_kernel(const float* __restrict__ xyz, FieldGrid g, long long p0, lo
       rdirs[3 * j] = d2[0]; rdirs[3 * j + 1] = d2[1]; rdirs[3 * j + 2] = d2[2];
     }
   }
-  // the edit part of march_point: p -= shift (layered_rfrender.py:298 / :471); p = (p - pivot)/scale + pivot (:303 / :475)
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    if (e.shift_on) v[a] = __fsub_rn(v[a], e.shift[a]);
-    if (e.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], e.pivot[a]), e.scale), e.pivot[a]);
-  }
+  inverse_edit(e, v);
   reinterpret_cast<float4*>(xyzt)[j] = make_float4(v[0], v[1], v[2], frame);
 }
 

@@ -367,7 +367,7 @@ constexpr int AUX_BIAS = 0, AUX_WSIG = 8 * 256, AUX_BSIG = AUX_WSIG + 256, AUX_W
 
 
 // ---------------------------------------------------------------------------------------------------------
-// point fetch (same arithmetic as mlp_simt.cu::fetch_point)
+// point fetch
 // ---------------------------------------------------------------------------------------------------------
 struct Pt { float x, y, z, tm; int out_index; int cidx; };
 
@@ -402,14 +402,8 @@ __device__ __forceinline__ Pt fetch_pt(const PointSrc& s, long long p, long long
     q.x = pp[0]; q.y = pp[1]; q.z = pp[2];
     return q;
   }
-  const float tt = s.t[ray * s.S + k];
-  float v[3] = {__fadd_rn(__fmul_rn(tt, rp[3]), rp[0]), __fadd_rn(__fmul_rn(tt, rp[4]), rp[1]),
-                __fadd_rn(__fmul_rn(tt, rp[5]), rp[2])};
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    if (s.shift_on) v[a] = __fsub_rn(v[a], s.shift[a]);
-    if (s.scale_on) v[a] = __fadd_rn(__fdiv_rn(__fsub_rn(v[a], s.pivot[a]), s.scale), s.pivot[a]);
-  }
+  float v[3];
+  march_point(s, rp, s.t[ray * s.S + k], rp[3], rp[4], rp[5], v);
   q.x = v[0]; q.y = v[1]; q.z = v[2];
   return q;
 }

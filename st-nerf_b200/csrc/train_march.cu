@@ -3,7 +3,7 @@
 // and the Philox uniforms of the fine resampling.
 //
 // Compiled with -fmad=false like geometry.cu / composite.cu: the marched points must round op by op like eager PyTorch
-// (they are march_point, shared with mlp_simt.cu's SRC_MARCH fetch), and the density masks and the alpha factor must give
+// (they are march_point, shared with the networks' SRC_MARCH fetch), and the density masks and the alpha factor must give
 // the very values composite_pass_kernel composites.
 #include "common.cuh"
 
