@@ -593,7 +593,7 @@ static int run_nets(stnerf_ctx* c, const LayerRays& rays, long long n, int ray_s
     memset(&f, 0, sizeof(f));
     if (fuse) {
       f = *fuse;
-      f.on = 1; f.layer = i; f.is_bkgd = (i == 0);
+      f.on = 1; f.layer = i;
       f.t_fine = c->t_fine + (size_t)i * R * c->cap_s2;
       f.z_new = fuse->z_new ? c->z_new + (size_t)i * R * c->cap_s2 : nullptr;
       f.src_map = fuse->z_new ? c->src_map + (size_t)i * R * c->cap_s2 : nullptr;
@@ -733,8 +733,7 @@ static int render_core(stnerf_ctx* c, const float* rays, long long n_rays, int r
     if (fuse) {
       ft.z_new = reuse ? c->z_new : nullptr;
       ft.n1 = n1; ft.n2 = n2; ft.u = u ? u + c0 * n2 : nullptr; ft.seed = seed; ft.idmap = c->idmap; ft.ray_base = c0;
-      ft.n_total = N; ft.pixels = out.pixels; ft.near_plane = c->dscene.near_plane; ft.thr = c->dscene.thr_layer;
-      ft.boarder = c->dscene.boarder; ft.apply_thr = c->dscene.apply_thr;
+      ft.n_total = N; ft.pixels = out.pixels; ft.mask = pass_mask(c->dscene); ft.boarder = c->dscene.boarder;
     }
     rc = run_nets(c, lr, n, ray_stride, false, n1, st, chunk_slot, fuse ? &ft : nullptr, /*want_raw=*/!fuse || out.coarse != nullptr,
                   out.coarse, 5 * N);

@@ -165,6 +165,37 @@ struct DevScene {
   int fid_shared;            // all layers read frame-id column 6 (7-column rays)
 };
 
+// The scene constants of the density masks of a pass (pass_sigma).
+struct PassMask {
+  float near_plane, alpha2, thr_layer, thr_bkgd;
+  int apply_thr;
+};
+__host__ __device__ inline PassMask pass_mask(const DevScene& s) { return {s.near_plane, s.alpha2, s.thr_layer, s.thr_bkgd, s.apply_thr}; }
+
+// The density of sample (t, sg) of `layer` after the masks of its pass (layered_rfrender.py:414-422 coarse, :538-547 /
+// :564-576 fine), as the compositing reads it.  factor: 0 (masked), alpha2 (layer 2, fine pass) or 1 -- torch's gradient of
+// `density[mask] = 0` and of `density *= alpha`, which the training scatter records.  A kept density keeps its bits: it is
+// not multiplied by 1 (a product may change a NaN's payload).
+__device__ __forceinline__ float pass_sigma(const PassMask& m, int layer, bool fine, float t, float sg, float& factor) {
+  float v = sg;
+  bool kept = true;
+  if (!fine) {
+    if (layer > 0) {
+      if (t < 0.0f) { v = 0.0f; kept = false; }                                       // :414
+      if (m.apply_thr && v < m.thr_layer) { v = 0.0f; kept = false; }                 // :416-418
+    } else if (t < m.near_plane) {
+      v = 0.0f; kept = false;                                                         // :422
+    }
+  } else if (layer == 0) {
+    if (m.apply_thr && v < m.thr_bkgd) { v = 0.0f; kept = false; }                    // :538-547
+  } else {
+    if (m.apply_thr && v < m.thr_layer) { v = 0.0f; kept = false; }                   // :564-566
+    if (layer == 2) v = v * m.alpha2;                                                 // :575-576
+  }
+  factor = !kept ? 0.0f : (fine && layer == 2) ? m.alpha2 : 1.0f;
+  return v;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Philox4x32-10 (production RNG when no uniforms are injected; statistically equivalent to torch.rand,
 // not bit-equal -- parity runs inject uniforms).

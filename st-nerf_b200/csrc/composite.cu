@@ -12,6 +12,9 @@
 namespace stnerf {
 
 constexpr unsigned FULL = 0xffffffffu;
+using rs::lower_bound_s;
+using rs::upper_bound_s;
+using rs::write_pixel;
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -61,17 +64,6 @@ __device__ __forceinline__ void warp_bitonic_sort(T* a, int P, int lane) {
   }
 }
 
-// first index with a[idx] >= key / > key in an ascending shared-memory array
-__device__ __forceinline__ int lower_bound_s(const float* a, int n, float key) {
-  int lo = 0, hi = n;
-  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
-  return lo;
-}
-__device__ __forceinline__ int upper_bound_s(const float* a, int n, float key) {
-  int lo = 0, hi = n;
-  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] <= key) lo = mid + 1; else hi = mid; }
-  return lo;
-}
 // warp-uniform: is a[0..n) non-decreasing?
 __device__ __forceinline__ bool warp_is_ascending(const float* a, int n, int lane) {
   bool ok = true;
@@ -123,15 +115,6 @@ __device__ __forceinline__ void composite_run(int count, At at, Rgb rgb_at, cons
   out[3] = warp_sum(cd); out[4] = warp_sum(ca);
 }
 
-// One image pixel (rgb, depth, acc) of ray `rg`: plane layout rgb (N,3) | depth (N) | acc (N), or 5 interleaved floats.
-__device__ __forceinline__ void write_pixel(float* img, long long rg, long long n_total, bool pixels, const float o5[5], int lane) {
-  if (img == nullptr || lane >= 5) return;
-  const float v = lane == 0 ? o5[0] : lane == 1 ? o5[1] : lane == 2 ? o5[2] : lane == 3 ? o5[3] : o5[4];
-  if (pixels) img[rg * 5 + lane] = v;
-  else if (lane < 3) img[rg * 3 + lane] = v;
-  else img[(long long)lane * n_total + rg] = v;
-}
-
 // utils/sample_pdf.py:18-63 for one ray: t[n1] (any order), w[n1] full weights, n2 uniforms -> z written to
 // zbuf[0..n2).  cdf is an (n1-1)-float scratch.
 template <typename U>
@@ -154,11 +137,7 @@ __device__ __forceinline__ void sample_pdf_ray(const float* s_t, const float* s_
   const int nc = n1 - 1;                      // len(cdf) == len(bins)
   for (int j = lane; j < n2; j += 32) {
     const float uu = get_u(j);
-    int lo = 0, hi = nc;                      // searchsorted(right=True): first index with cdf > u (:47)
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (cdf[mid] <= uu) lo = mid + 1; else hi = mid;
-    }
+    const int lo = upper_bound_s(cdf, nc, uu);                                     // :47
     const int below = max(lo - 1, 0);                                              // :48
     const int above = min(lo, nc - 1);                                             // :49
     const float cb = cdf[below], ca = cdf[above];
@@ -222,7 +201,7 @@ __global__ void __launch_bounds__(256, 3) composite_pass_kernel(const CompositeA
   const int S = a.S, n2 = a.n2;
   const bool fine = a.fine != 0;
   const float near_p = scene.near_plane, boarder = scene.boarder;
-  const bool thr_on = scene.apply_thr != 0;
+  const PassMask pm = pass_mask(scene);
   const long long plane = 5 * a.n_total;
   const bool pixels = a.pixel_layout != 0;
   unsigned shown_mask = 1u;
@@ -250,25 +229,8 @@ __global__ void __launch_bounds__(256, 3) composite_pass_kernel(const CompositeA
       const float4* rp = reinterpret_cast<const float4*>(a.raw + i * a.raw_layer_stride) + r * S;
       for (int k = lane; k < S; k += 32) {
         const float tk = tp[k];
-        float sg = 0.f;
-        if (shown) {
-          sg = rp[k].w;
-          if (!fine) {
-            if (i > 0) {
-              if (tk < 0.0f) sg = 0.0f;                                         // layered_rfrender.py:414
-              if (thr_on && sg < scene.thr_layer) sg = 0.0f;                   // :416-418
-            } else if (tk < near_p) {
-              sg = 0.0f;                                                        // :422
-            }
-          } else {
-            if (i == 0) {
-              if (thr_on && sg < scene.thr_bkgd) sg = 0.0f;                    // :538-547
-            } else {
-              if (thr_on && sg < scene.thr_layer) sg = 0.0f;                   // :564-566
-              if (i == 2) sg = sg * scene.alpha2;                              // :575-576
-            }
-          }
-        }
+        float sg = 0.f, factor;
+        if (shown) sg = pass_sigma(pm, i, fine, tk, rp[k].w, factor);
         s_t[off + k] = tk;
         s_sig[off + k] = sg;
       }

@@ -560,16 +560,9 @@ __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float
 #pragma unroll
       for (int s = 0; s < 2; ++s) {
         const int k = s * 32 + lane;
-        const float tk = __ldg(tp + k);
-        float v = rp[k].w;
-        if (F.is_bkgd) {
-          if (tk < F.near_plane) v = 0.0f;                                     // layered_rfrender.py:422
-        } else {
-          if (tk < 0.0f) v = 0.0f;                                              // :414
-          if (F.apply_thr && v < F.thr) v = 0.0f;                               // :416-418
-        }
-        t[s] = tk;
-        sg[s] = v;
+        float factor;
+        t[s] = __ldg(tp + k);
+        sg[s] = pass_sigma(F.mask, F.layer, false, t[s], rp[k].w, factor);
       }
       const float* up = F.u ? F.u + ray * n2 : nullptr;
       const uint64_t seed = F.seed;
@@ -586,13 +579,7 @@ __device__ __noinline__ void fused_composite_loop(const TcParams& P, const float
           [up, seed, stream, gid](int jj) { return up ? up[jj] : philox_uniform(seed, stream, gid, (uint32_t)jj); },
           cdf, F.t_fine + ray * (n1 + n2), lane, lo, F.z_new ? F.z_new + ray * n2 : nullptr,
           F.z_new ? F.src_map + ray * (n1 + n2) : nullptr);
-      if (F.img && lane < 5) {
-        const long long rg = F.ray_base + ray;
-        const float v = lane == 0 ? lo.pix[0] : lane == 1 ? lo.pix[1] : lane == 2 ? lo.pix[2] : lane == 3 ? lo.pix[3] : lo.pix[4];
-        if (F.pixels) F.img[rg * 5 + lane] = v;
-        else if (lane < 3) F.img[rg * 3 + lane] = v;
-        else F.img[(long long)lane * F.n_total + rg] = v;
-      }
+      rs::write_pixel(F.img, F.ray_base + ray, F.n_total, F.pixels, lo.pix, lane);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(bar_empty);

@@ -11,7 +11,7 @@ namespace stnerf {
 // tile's MMAs.  Arithmetic: resample.cuh, shared with the stand-alone compositing kernel.
 struct FuseCoarse {
   int on;                      // 0: the kernel only evaluates the network
-  int n1, n2, layer, is_bkgd;
+  int n1, n2, layer;
   const float* u;              // injected uniforms of this layer, [ray][n2], or null -> Philox(seed, 64 + layer, ray id, j)
   uint64_t seed;
   RayIdMap idmap;
@@ -22,8 +22,8 @@ struct FuseCoarse {
   float* img;                  // out: this layer's coarse image (one pixel per hit ray), or null
   long long n_total;           // rays of the whole call (plane geometry of img)
   int pixels;                  // img layout: 0 planes, 1 pixel-interleaved
-  float near_plane, thr, boarder;
-  int apply_thr;
+  PassMask mask;               // density masks of the coarse pass (pass_sigma)
+  float boarder;
 };
 
 // Weights of one network packed for the tensor-core kernels (see mlp_tc.cu for the layout).

@@ -41,6 +41,27 @@ __device__ __forceinline__ float wscan_add(float v, int lane) {
   return v;
 }
 
+// first index with a[idx] >= key / > key in an ascending array (torch.searchsorted, right=False / True)
+__device__ __forceinline__ int lower_bound_s(const float* a, int n, float key) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+__device__ __forceinline__ int upper_bound_s(const float* a, int n, float key) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] <= key) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+
+// One image pixel (rgb, depth, acc) of ray `rg`: plane layout rgb (N,3) | depth (N) | acc (N), or 5 interleaved floats.
+__device__ __forceinline__ void write_pixel(float* img, long long rg, long long n_total, bool pixels, const float o5[5], int lane) {
+  if (img == nullptr || lane >= 5) return;
+  const float v = lane == 0 ? o5[0] : lane == 1 ? o5[1] : lane == 2 ? o5[2] : lane == 3 ? o5[3] : o5[4];
+  if (pixels) img[rg * 5 + lane] = v;
+  else if (lane < 3) img[rg * 3 + lane] = v;
+  else img[(long long)lane * n_total + rg] = v;
+}
+
 // value of striped element `idx` (lane idx % 32, slot idx / 32) of a register array; every lane must call it
 template <int N>
 __device__ __forceinline__ float gather(const float (&v)[N], int idx) {
@@ -184,11 +205,7 @@ __device__ __forceinline__ void composite_resample_ray(const float (&t)[NT], con
   for (int q = 0; q < NZ; ++q) {
     const int j = q * 32 + lane;
     const float uu = (j < n2) ? get_u(j) : 0.f;
-    int lo = 0, hi = nc;                      // searchsorted(right=True): first index with cdf > u (:47)
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (cdf[mid] <= uu) lo = mid + 1; else hi = mid;
-    }
+    const int lo = upper_bound_s(cdf, nc, uu);                                           // :47
     const int below = max(lo - 1, 0);                                                    // :48
     const int above = min(lo, nc - 1);                                                   // :49
     const float cbv = cdf[below], cav = cdf[above];
@@ -219,12 +236,7 @@ __device__ __forceinline__ void composite_resample_ray(const float (&t)[NT], con
       const int e = q * 32 + lane;
       if (e < n2) {
         const float key = z[q];
-        int lo = 0, hi = n1;                                     // upper bound: first index with t > key
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (cdf[mid] <= key) lo = mid + 1; else hi = mid;
-        }
-        const int pos = e + lo;
+        const int pos = e + upper_bound_s(cdf, n1, key);
         tf[pos] = key;
         if (zs != nullptr) { zs[e] = key; src[pos] = (uint8_t)(n1 + e); }
 #pragma unroll

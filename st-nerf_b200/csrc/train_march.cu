@@ -132,26 +132,11 @@ int launch_train_points(const PointSrc& s, long long P, float* pos, float* dirs,
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Masked scatter.  The density masks of one pass exactly as composite_pass_kernel applies them (layered_rfrender.py:414-422
-// coarse, :538-547 / :564-576 fine): factor 0 (masked), alpha2 (layer 2, fine pass) or 1.  The forward writes
-// factor * sigma (sigma itself when the factor is 1, so the bits are the composite kernel's) and records the factor; the
-// backward multiplies the dense gradient by it -- torch's gradient of `density[mask] = 0` and of `density *= alpha`.
+// Masked scatter: the density of one pass and layer as composite_pass_kernel composites it and the factor of its mask
+// (pass_sigma); the backward multiplies the dense gradient by that factor.
 // ---------------------------------------------------------------------------------------------------------
-struct PassMask {
-  float near_plane, alpha2, thr_layer, thr_bkgd;
-  int apply_thr, layer, fine;
-};
-
-__device__ __forceinline__ bool pass_keeps(const PassMask& m, float sg, float tk) {
-  if (!m.fine) {
-    if (m.layer > 0) return !(tk < 0.0f) && !(m.apply_thr && sg < m.thr_layer);
-    return !(tk < m.near_plane);
-  }
-  if (m.layer == 0) return !(m.apply_thr && sg < m.thr_bkgd);
-  return !(m.apply_thr && sg < m.thr_layer);
-}
-
-__global__ void train_scatter_kernel(const PassMask m, const float* __restrict__ t, int S, const int* __restrict__ hit, long long P,
+__global__ void train_scatter_kernel(const PassMask m, int layer, int fine, const float* __restrict__ t, int S,
+                                     const int* __restrict__ hit, long long P,
                                      const float* __restrict__ rgb_c, const float* __restrict__ sigma_c, float* __restrict__ rgb,
                                      float* __restrict__ sigma, float* __restrict__ factor) {
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -160,11 +145,8 @@ __global__ void train_scatter_kernel(const PassMask m, const float* __restrict__
   const int k = (int)(p - slot * S);
   const long long ray = hit ? (long long)hit[slot] : slot;
   const long long q = ray * S + k;
-  const float sg = sigma_c[p];
-  float f = pass_keeps(m, sg, t[q]) ? 1.0f : 0.0f;
-  float v = f != 0.0f ? sg : 0.0f;
-  if (m.fine && m.layer == 2 && f != 0.0f) { v = v * m.alpha2; f = m.alpha2; }      // :575-576
-  sigma[q] = v;
+  float f;
+  sigma[q] = pass_sigma(m, layer, fine, t[q], sigma_c[p], f);
   rgb[3 * q] = rgb_c[3 * p]; rgb[3 * q + 1] = rgb_c[3 * p + 1]; rgb[3 * q + 2] = rgb_c[3 * p + 2];
   if (factor) factor[p] = f;
 }
@@ -190,8 +172,8 @@ int launch_train_scatter(const DevScene& sc, int layer, int fine, const float* t
   STNERF_CUDA(cudaMemsetAsync(rgb, 0, (size_t)n * S * 3 * sizeof(float), st));        // rays that miss the box: zeros
   STNERF_CUDA(cudaMemsetAsync(sigma, 0, (size_t)n * S * sizeof(float), st));
   if (P <= 0) return STNERF_OK;
-  PassMask m{sc.near_plane, sc.alpha2, sc.thr_layer, sc.thr_bkgd, sc.apply_thr, layer, fine};
-  train_scatter_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(m, t, S, hit, P, rgb_c, sigma_c, rgb, sigma, factor);
+  train_scatter_kernel<<<(int)((P + 255) / 256), 256, 0, st>>>(pass_mask(sc), layer, fine, t, S, hit, P, rgb_c, sigma_c, rgb, sigma,
+                                                               factor);
   STNERF_LAUNCH_CHECK();
   return STNERF_OK;
 }
